@@ -124,7 +124,9 @@ class acgb200_info(C.Structure):
                                                                                   ("spmv_merge_tiles", C.c_int),
                                                                                   ("spmv_merge_rows", C.c_int),
                                                                                   ("spmv_merge_split", C.c_int),
-                                                                                  ("spmv_slice_exc", C.c_int)]
+                                                                                  ("spmv_slice_exc", C.c_int)] + \
+        [(n, C.c_int) for n in ("spmv_threads", "spmv_unroll", "spmv_slice_threads", "spmv_merge_threads",
+                                "spmv_merge_grid", "spmv_merge_stages")]
 
 
 class acgb200_mtxinfo(C.Structure):
@@ -151,7 +153,7 @@ EXPORTS = [
     "acgsolvercuda_init_constants", "acgsolvercuda_alpha", "acgsolvercuda_beta", "acgsolvercuda_daxpy_alpha",
     "acgsolvercuda_daxpy_minus_alpha", "acgsolvercuda_daypx_beta", "acgsolvercuda_pipelined_daxpy_fused",
     "acgsolvercuda_fwrite",
-    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
+    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
     "acgb200_nccl_unique_id", "acgb200_comm_init_rank", "acgb200_comm_destroy",
     "acgb200_host_register", "acgb200_host_unregister", "acgb200_spmv_plan_host", "acgb200_spmv_plan_host2", "acgb200_slices_host", "acgb200_merge_plan_host", "acgb200_p2p_inverse_map", "acgb200_patterns_host", "acgb200_stencil_part",
     "acgb200_mtx_info", "acgb200_mtx_read", "acgb200_mtx_read_part", "acgb200_comm_matrix_row", "acgb200_partition_rows_grid", "acgb200_grid_factors", "acgb200_rmat_spd",
@@ -229,6 +231,7 @@ def lib() -> C.CDLL:
     L.acgsolvercuda_fwrite.argtypes = [C.c_void_p, P(acgsolvercuda), C.c_int]
     L.acgsolvercuda_spmv.argtypes = [P(acgsolvercuda), f64p, f64p, C.c_int, P(C.c_double)]
     L.acgsolvercuda_spmv_ghost.argtypes = [P(acgsolvercuda), f64p, f64p, C.c_int, P(C.c_double)]
+    L.acgsolvercuda_spmv_mode.argtypes = [P(acgsolvercuda), C.c_int, f64p, C.c_void_p, f64p, C.c_int, P(C.c_double)]
     L.acgsolvercuda_info.argtypes = [P(acgsolvercuda), P(acgb200_info)]
     L.acgb200_set_option.argtypes = [C.c_char_p, C.c_int]
     L.acgb200_nccl_unique_id.argtypes = [C.c_void_p]
@@ -675,6 +678,26 @@ class SolverCuda:
         y = np.zeros(self.A.c.nownedrows, np.float64)
         dot = C.c_double(0)
         _check(lib().acgsolvercuda_spmv_ghost(C.byref(self.c), x, y, path, C.byref(dot)), "acgsolvercuda_spmv_ghost")
+        return y, dot.value
+
+    SPMV_Y_AX, SPMV_Y_AX_DOT, SPMV_R_B_AX = 0, 1, 2
+
+    def spmv_mode(self, mode: int, x: np.ndarray, b: np.ndarray | None = None, path: int = 0):
+        """The product in one of the SpMV epilogue modes (acgsolvercuda_spmv_mode): mode 0 y = A x,
+        1 y = A x with dot = x.y, 2 y = b - A x with dot = y.y.  x has the owned + ghost entries,
+        b the owned rows (mode 2).  Returns (y over the owned rows, fused dot)."""
+        x = np.ascontiguousarray(x, np.float64)
+        assert len(x) == self.c.r.num_nonzeros
+        no = self.A.c.nownedrows
+        bp = None
+        if b is not None:
+            b = np.ascontiguousarray(b, np.float64)
+            assert len(b) == no
+            bp = b.ctypes.data_as(C.c_void_p)
+        y = np.zeros(no, np.float64)
+        dot = C.c_double(0)
+        _check(lib().acgsolvercuda_spmv_mode(C.byref(self.c), int(mode), x, bp, y, int(path), C.byref(dot)),
+               "acgsolvercuda_spmv_mode")
         return y, dot.value
 
     def info(self) -> dict:

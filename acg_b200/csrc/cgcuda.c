@@ -795,6 +795,14 @@ static double evpool_sum_ms(struct evpool *p)
     return tot;
 }
 
+/* offdiag_kernel's share of the epilogue of `mode` (o->acc set): add the border x ghost block to
+ * y = A x, or subtract it from r = b - A x; dot over the finished rows as the SpMV kernels form it */
+static void offdiag_epilogue(struct acgb200_offdiagargs *o, int mode)
+{
+    o->minus = (mode == SPMV_R_B_AX);
+    o->dotkind = !o->acc ? 0 : (mode == SPMV_R_B_AX ? 2 : (mode == SPMV_Y_AX_DOT ? 1 : 0));
+}
+
 /* y = A x (or r = b - A x) over owned rows, including the halo exchange of x
  * and the border x ghost block when the matrix is distributed.  `acc` gets the
  * fused dot.  `gated`: take part in the device-side iteration control. */
@@ -859,8 +867,7 @@ static int apply_A(struct solvectx *c, const double *x_ro, double *x_halo, doubl
         o.nrows = pv->nborder; o.rowoffset = pv->borderoff;
         o.orowptr = cg->d_orowptr; o.ocolidx = cg->d_ocolidx; o.oa = cg->d_oa;
         o.x = x_ro; o.y = y; o.acc = acc;
-        o.minus = (mode == SPMV_R_B_AX);
-        o.dotkind = !acc ? 0 : (mode == SPMV_R_B_AX ? 2 : (mode == SPMV_Y_AX_DOT ? 1 : 0));
+        offdiag_epilogue(&o, mode);
         if (gated) o.ctrl_in = &pv->d_st->ctrl[1];
         o.st = pv->d_st;
         o.p2p = peer ? pv->p2p.d_desc : NULL; o.p2p_iter_override = -1;
@@ -1651,29 +1658,39 @@ int acgsolvercuda_spmv(struct acgsolvercuda *cg, const double *x, double *y, int
 }
 
 /*
- * One part's share of y = A x on ONE device, ghost values supplied by the caller: x has the
- * part's nvec = owned + ghost entries, y its owned rows.  path 0 is what the set-up products and
- * the NCCL loop back-end run (local block through the tile kernel, then offdiag_kernel adding
- * the border x ghost block from the ghost tail of x: acg/cgcuda.c:858 + :878); path 1 is the
- * kernel of the peer-memory loop: border x ghost block inside the tile kernel, ghost values read
- * from a window whose senders' flags are waited for (here a loop-back window in this device's
- * memory, filled from x's tail, the flags already published).  *dot = sum_owned x_i y_i from the
- * fused epilogue.  Needs no communicator -- it exists so that the border x ghost path of a
- * partitioned matrix can be checked against the global product on a single GPU.
+ * One part's share of the product on ONE device in any of the three epilogue modes, ghost values
+ * supplied by the caller: x has the part's nvec = owned + ghost entries, b (mode 2 only) and y its
+ * owned rows.  mode 0: y = A x; mode 1: y = A x and *dot = sum_owned x_i y_i; mode 2: y = b - A x
+ * and *dot = sum_owned y_i^2 -- the fused dots as the solver's epilogues compute them (mode 0
+ * passes the accumulator too, which must stay 0).  path 0 is what the set-up products and the NCCL
+ * loop back-end run (local block through the SpMV kernels, then offdiag_kernel adding -- or, in
+ * mode 2, subtracting -- the border x ghost block from the ghost tail of x: acg/cgcuda.c:858 +
+ * :878); path 1 is the kernel of the peer-memory loop: border x ghost block inside the tile kernel,
+ * ghost values read from a window whose senders' flags are waited for (here a loop-back window in
+ * this device's memory, filled from x's tail, the flags already published).  Whole matrices (no
+ * ghosts) take either path.  y is poisoned before the launch, so a row no kernel writes reads NaN.
+ * Needs no communicator -- it exists so that every kernel's epilogues and the border x ghost path
+ * of a partitioned matrix can be checked against exact products on a single GPU.
  */
-int acgsolvercuda_spmv_ghost(struct acgsolvercuda *cg, const double *x, double *y, int path, double *dot)
+int acgsolvercuda_spmv_mode(struct acgsolvercuda *cg, int mode, const double *x, const double *b, double *y,
+                            int path, double *dot)
 {
     int errcode_ = 0, *errcode = &errcode_;
     struct priv *pv = priv_of(cg);
     if (!pv || (path != 0 && path != 1)) return ACG_ERR_INVALID_VALUE;
+    if (mode != SPMV_Y_AX && mode != SPMV_Y_AX_DOT && mode != SPMV_R_B_AX) return ACG_ERR_INVALID_VALUE;
+    if (mode == SPMV_R_B_AX && !b) return ACG_ERR_INVALID_VALUE;
     const int n = pv->nowned;
     struct acgb200_devstate *st = pv->d_st;
     CU(cudaMemcpyAsync(cg->d_p, x, (size_t) pv->nvec * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
+    if (mode == SPMV_R_B_AX) CU(cudaMemcpyAsync(cg->d_r, b, (size_t) n * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
+    CU(cudaMemsetAsync(cg->d_t, 0xff, (size_t) n * sizeof(double), pv->stream));
     CU(cudaMemsetAsync(&st->tmp_loc[0], 0, sizeof(double), pv->stream));
     struct acgb200_spmvargs a;
     memset(&a, 0, sizeof(a));
     a.plan = &pv->plan; a.rowptr = cg->d_rowptr; a.colidx = cg->d_colidx; a.a = cg->d_a;
-    a.x = cg->d_p; a.y = cg->d_t; a.mode = SPMV_Y_AX_DOT; a.acc = &st->tmp_loc[0]; a.dotrows = n; a.pub_ch = -1;
+    a.x = cg->d_p; a.y = cg->d_t; a.b = mode == SPMV_R_B_AX ? cg->d_r : NULL;
+    a.mode = mode; a.acc = &st->tmp_loc[0]; a.dotrows = n; a.pub_ch = -1;
     void *d_win = NULL;
     if (path == 0) {
         a.dotrows = pv->borderoff;                  /* the border rows' share of the dot comes from offdiag_kernel */
@@ -1682,7 +1699,8 @@ int acgsolvercuda_spmv_ghost(struct acgsolvercuda *cg, const double *x, double *
         memset(&o, 0, sizeof(o));
         o.nrows = pv->nborder; o.rowoffset = pv->borderoff;
         o.orowptr = cg->d_orowptr; o.ocolidx = cg->d_ocolidx; o.oa = cg->d_oa;
-        o.x = cg->d_p; o.y = cg->d_t; o.acc = &st->tmp_loc[0]; o.dotkind = 1; o.st = st; o.p2p_iter_override = -1;
+        o.x = cg->d_p; o.y = cg->d_t; o.acc = &st->tmp_loc[0]; o.st = st; o.p2p_iter_override = -1;
+        offdiag_epilogue(&o, mode);
         KL(acgb200_offdiag_launch(&o, pv->stream));
     } else {
         /* loop-back window: [descriptor | flags (one per sender slot) | ghost values] */
@@ -1728,6 +1746,11 @@ int acgsolvercuda_spmv_ghost(struct acgsolvercuda *cg, const double *x, double *
     return ACG_SUCCESS;
 }
 
+int acgsolvercuda_spmv_ghost(struct acgsolvercuda *cg, const double *x, double *y, int path, double *dot)
+{
+    return acgsolvercuda_spmv_mode(cg, SPMV_Y_AX_DOT, x, NULL, y, path, dot);
+}
+
 int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info)
 {
     const struct priv *pv = priv_of(cg);
@@ -1748,6 +1771,10 @@ int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info
     info->spmv_slice_exc = (int) pv->plan.slice_exc;
     info->spmv_slice_ub = pv->plan.slice_ub; info->spmv_slice_grid = pv->plan.slice_grid;
     info->spmv_nmedium = pv->plan.nmed;
+    info->spmv_threads = pv->plan.threads; info->spmv_unroll = pv->plan.unroll;
+    info->spmv_slice_threads = pv->plan.slice_threads;
+    info->spmv_merge_threads = pv->plan.merge_threads; info->spmv_merge_grid = pv->plan.merge_grid;
+    info->spmv_merge_stages = pv->plan.merge_stages;
     info->spmv_min_bytes = acgb200_spmv_min_bytes(&pv->plan);
     return ACG_SUCCESS;
 }

@@ -41,6 +41,15 @@ ACG_API int acgsolvercuda_spmv(struct acgsolvercuda *cg, const double *x, double
  * single-GPU parity tests of the border x ghost path of partitioned matrices. */
 ACG_API int acgsolvercuda_spmv_ghost(struct acgsolvercuda *cg, const double *x, double *y, int path, double *dot);
 
+/* The same product in any of the solver's three SpMV epilogue modes (acgsolvercuda_spmv_ghost is
+ * mode 1): mode 0 y = A x; mode 1 y = A x and *dot = sum_owned x_i y_i; mode 2 y = b - A x and
+ * *dot = sum_owned y_i^2 (b: owned rows, host; may be NULL otherwise).  *dot (may be NULL) is the
+ * fused accumulator as the kernels leave it -- 0 in mode 0.  path as above; a whole matrix (no
+ * ghosts) takes either.  y is poisoned on the device first, so a row nobody writes comes back NaN.
+ * For tests of every SpMV kernel's epilogues against exact products. */
+ACG_API int acgsolvercuda_spmv_mode(struct acgsolvercuda *cg, int mode, const double *x, const double *b, double *y,
+                                    int path, double *dot);
+
 struct acgb200_info {
     int spmv_lanes_per_row, spmv_rows_cap, spmv_nnz_cap, spmv_stages;
     int spmv_ntiles, spmv_nlong, spmv_grid, spmv_smem_bytes;
@@ -64,6 +73,9 @@ struct acgb200_info {
     int spmv_merge_rows;        /* ... the rows [0, spmv_merge_rows) they cover ... */
     int spmv_merge_split;       /* ... and the rows cut by tile boundaries (finished by spmv_merge_fix_kernel) */
     int spmv_slice_exc;         /* rows inside slices that are not in the pattern dictionary (columns from the index array) */
+    int spmv_threads, spmv_unroll;              /* shape of the tile kernel (with spmv_lanes_per_row) */
+    int spmv_slice_threads;                     /* CTA size of the slice kernel (with spmv_slice_ub) */
+    int spmv_merge_threads, spmv_merge_grid, spmv_merge_stages;    /* shape and grid of the merge-path kernel */
 };
 ACG_API int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info);
 

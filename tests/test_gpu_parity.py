@@ -488,3 +488,92 @@ def test_public_blas1_building_blocks(ab):
         assert L.acgsolvercuda_daxpy_alpha(1, q.value, p1.value, p1.value, got[i:i + 1].data_ptr()) == 0    # got[i] += (q/1)*1
     torch.cuda.synchronize()
     assert got.cpu().tolist() == [-1.0, 1.0, 0.0]
+
+
+# ---- nonzero initial guesses ------------------------------------------------------------------
+# With x0 = 0 the set-up product r0 = b - A x0 is b - 0: a wrong sign or a wrong b[row] in an epilogue of mode
+# r = b - A x, or a warm-up that clobbers x0, would go unnoticed.  These solves start elsewhere.
+
+def _laplacian_values(n, r, c):
+    """off-diagonal -1, diagonal 1 + degree: symmetric, strictly diagonally dominant"""
+    off = r != c
+    deg = np.bincount(r[off], minlength=n) + np.bincount(c[off], minlength=n)
+    v = np.where(off, -1.0, 0.0)
+    v[~off] = 1.0 + deg[r[~off]]
+    return v
+
+
+def _x0_plan(name):
+    from test_gpu_kernel_variants import slice_matrix
+    if name == "tiles":
+        return mg.stencil3d_27pt(10, 9, 11), dict(spmv_slices=0, spmv_merge=0)
+    if name == "slices":
+        return mg.stencil3d_27pt(10, 9, 11), {}
+    if name == "slices-exc":
+        n, r, c = slice_matrix(True)
+        return (n, r, c, _laplacian_values(n, r, c)), {}
+    if name == "merge":
+        return mg.rmat_spd(6000, 60000, seed=3), dict(spmv_merge=1, spmv_slices=0, merge_items=256)
+    if name == "medium+long":
+        return mg.rmat_spd(30000, 600000, seed=8), dict(spmv_medium=96, spmv_merge=0)
+    raise ValueError(name)
+
+
+X0_PLANS = ["tiles", "slices", "slices-exc", "merge", "medium+long"]
+X0_ENTRIES = [("solvempi", "cg"), ("solve_pipelined", "cg_pipelined"), ("solve_device", "cg"),
+              ("solve_device_pipelined", "cg_pipelined"), ("solve", "cg")]
+_X0_DEFAULTS = {"spmv_slices": 1, "spmv_merge": -1, "merge_items": 0, "spmv_medium": 0}
+
+
+@pytest.mark.parametrize("plan", X0_PLANS)
+def test_nonzero_initial_guess(plan, ab, oracle):
+    """All five entry points, warm-up 0 and 2, from a random x0 (against the oracle started from the same x0),
+    from an x0 next to the solution (r0nrm2 against the exact ||b - A x0||) and with maxits = 0 (x comes back
+    bitwise as x0)."""
+    from exactref import gamma, rows_exact
+    (n, r, c, v), opts = _x0_plan(plan)
+    for k, val in opts.items():
+        ab.set_option(k, val)
+    try:
+        A, cg = _solver(ab, n, r, c, v)
+    finally:
+        for k in opts:
+            ab.set_option(k, _X0_DEFAULTS[k])
+    inf = cg.info()
+    assert {"tiles": inf["spmv_slices"] == 0 and inf["spmv_merge_tiles"] == 0 and inf["spmv_ntiles"] > 0,
+            "slices": inf["spmv_slices"] > 0 and inf["spmv_slice_exc"] == 0,
+            "slices-exc": inf["spmv_slice_exc"] > 0,
+            "merge": inf["spmv_merge_tiles"] > 0 and inf["spmv_merge_split"] > 0,
+            "medium+long": inf["spmv_nmedium"] > 0 and inf["spmv_nlong"] > 0}[plan], inf
+    csr = (A.frowptr.copy(), A.fcolidx.copy(), A.fa.copy())
+    rng = np.random.default_rng(21)
+    b = A.vector(); b.x[:] = rng.standard_normal(n)
+    x0 = rng.standard_normal(n)
+    # the power-law matrices are ill conditioned: compare after a fixed number of iterations (as above)
+    fixed = plan in ("merge", "medium+long")
+    its, rtol, xtol = (10, 0.0, 1e-7) if fixed else (300, 1e-9, 1e-9)
+    xs = rng.standard_normal(n)
+    bs = A.vector(); bs.x[:] = rows_exact(*csr, xs)[0]
+    xnear = xs + 1e-10 * rng.standard_normal(n)
+    rexact, rscale, m = rows_exact(*csr, xnear, bs.x)
+    for entry, oname in X0_ENTRIES:
+        want = getattr(oracle, oname)(csr, b.x, x0=x0, maxits=its, rtol=rtol)
+        for warmup in (0, 2):
+            tag = (plan, entry, warmup)
+            x = A.vector(); x.x[:] = x0
+            code = getattr(cg, entry)(b, x, maxits=its, residualrtol=rtol, warmup=warmup)
+            assert code == want["status"] == 0, tag
+            assert cg.c.niterations == want["niterations"], tag
+            assert cg.c.r0nrm2 == pytest.approx(want["r0nrm2"], rel=1e-13), tag
+            assert cg.c.rnrm2 / cg.c.r0nrm2 == pytest.approx(want["rnrm2"] / want["r0nrm2"], rel=1e-6, abs=RES_RTOL), tag
+            assert np.abs(x.x - want["x"]).max() <= xtol * np.abs(want["x"]).max(), tag
+            # next to the solution: r0 = b - A x0 is 1e-9 of b, the exact norm is known
+            x = A.vector(); x.x[:] = xnear
+            getattr(cg, entry)(bs, x, maxits=1, warmup=warmup)
+            bound = np.linalg.norm(2.0 * gamma(m + 1) * rscale)
+            assert abs(cg.c.r0nrm2 - np.linalg.norm(rexact)) <= bound, (tag, cg.c.r0nrm2, np.linalg.norm(rexact), bound)
+            # no iteration: x0 comes back untouched, whatever the warm-up did
+            x = A.vector(); x.x[:] = x0
+            assert getattr(cg, entry)(b, x, maxits=0, warmup=warmup) in (0, 39) and cg.c.niterations == 0, tag
+            assert np.array_equal(x.x, x0), tag
+    cg.free()

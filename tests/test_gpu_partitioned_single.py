@@ -192,3 +192,44 @@ def test_collectives_over_one_rank_nccl(ab, oracle, torch_cuda):
         assert np.abs(x.x - want["x"]).max() <= 1e-10 * np.abs(want["x"]).max()
     cg.free()
     comm.destroy()
+
+
+@pytest.mark.parametrize("name,gen,pkind,nparts,dims", CASES, ids=[c[0] for c in CASES])
+def test_border_ghost_residual_mode_of_every_part(name, gen, pkind, nparts, dims, ab, oracle):
+    """r = b - A x with the fused r.r (the set-up product of a solve from x0 != 0) and y = A x without a dot,
+    on both device paths of every part: offdiag_kernel then SUBTRACTS the border x ghost block and folds r_i^2
+    into the dot (path 0), the fused kernels do both for the border rows (path 1).  Against the correctly
+    rounded global product (tests/exactref.py), b = A x + 1e-8 noise so that the subtraction cancels."""
+    from exactref import dot_exact, gamma, rows_exact
+    n, r, c, v = gen()
+    A = ab.SymCsrMatrix.init_real_double(n, r, c, v)
+    csr = oracle.full_csr(n, r, c, v)
+    rng = np.random.default_rng(9)
+    xg = rng.standard_normal(n)
+    yx, yscale, m = rows_exact(*csr, xg)
+    bg = yx + 1e-8 * rng.standard_normal(n)
+    rx, rscale, _ = rows_exact(*csr, xg, bg)
+    parts = A.partition(nparts, _rowparts(pkind, n, nparts, dims))
+    for p, pm in enumerate(parts):
+        pm.dsymv_init(0.0)
+        no, nv = pm.c.nownedrows, pm.c.nprows
+        gl = pm.nzrows[:nv].astype(np.int64)
+        assert pm.c.nborderrows > 0
+        cg = ab.SolverCuda(pm)
+        xl = xg[gl]
+        own = gl[:no]
+        for path in (0, 1):
+            for mode, want, scale in ((0, yx, yscale), (2, rx, rscale)):
+                tag = (name, p, path, mode)
+                y, dot = cg.spmv_mode(mode, xl, bg[own] if mode == 2 else None, path)
+                err = np.abs(y - want[own])
+                bound = 2.0 * gamma(m[own] + 1) * scale[own]
+                assert np.all(err <= bound), (tag, float((err - bound).max()))
+                if mode == 0:
+                    assert dot == 0.0, tag
+                else:
+                    assert abs(dot - dot_exact(y, y)) <= 2.0 * gamma(no) * float(y @ y), (tag, dot, dot_exact(y, y))
+        cg.free()
+    for pm in parts:
+        pm.free()
+    A.free()
