@@ -126,7 +126,13 @@ class acgb200_info(C.Structure):
                                                                                   ("spmv_merge_split", C.c_int),
                                                                                   ("spmv_slice_exc", C.c_int)] + \
         [(n, C.c_int) for n in ("spmv_threads", "spmv_unroll", "spmv_slice_threads", "spmv_merge_threads",
-                                "spmv_merge_grid", "spmv_merge_stages")]
+                                "spmv_merge_grid", "spmv_merge_stages")] + \
+        [("spmv_slice_value_bytes", C.c_int64), ("spmv_slice_nnz", C.c_int64)]
+
+
+class acgb200_colstats(C.Structure):
+    _fields_ = [("niterations", C.c_int), ("converged", C.c_int), ("bnrm2", C.c_double), ("r0nrm2", C.c_double),
+                ("rnrm2", C.c_double)]
 
 
 class acgb200_mtxinfo(C.Structure):
@@ -153,7 +159,7 @@ EXPORTS = [
     "acgsolvercuda_init_constants", "acgsolvercuda_alpha", "acgsolvercuda_beta", "acgsolvercuda_daxpy_alpha",
     "acgsolvercuda_daxpy_minus_alpha", "acgsolvercuda_daypx_beta", "acgsolvercuda_pipelined_daxpy_fused",
     "acgsolvercuda_fwrite",
-    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
+    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_solve_multi", "acgsolvercuda_spmm_mode", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
     "acgb200_nccl_unique_id", "acgb200_comm_init_rank", "acgb200_comm_destroy",
     "acgb200_host_register", "acgb200_host_unregister", "acgb200_spmv_plan_host", "acgb200_spmv_plan_host2", "acgb200_slices_host", "acgb200_merge_plan_host", "acgb200_p2p_inverse_map", "acgb200_patterns_host", "acgb200_stencil_part",
     "acgb200_mtx_info", "acgb200_mtx_read", "acgb200_mtx_read_part", "acgb200_comm_matrix_row", "acgb200_partition_rows_grid", "acgb200_grid_factors", "acgb200_rmat_spd",
@@ -232,6 +238,9 @@ def lib() -> C.CDLL:
     L.acgsolvercuda_spmv.argtypes = [P(acgsolvercuda), f64p, f64p, C.c_int, P(C.c_double)]
     L.acgsolvercuda_spmv_ghost.argtypes = [P(acgsolvercuda), f64p, f64p, C.c_int, P(C.c_double)]
     L.acgsolvercuda_spmv_mode.argtypes = [P(acgsolvercuda), C.c_int, f64p, C.c_void_p, f64p, C.c_int, P(C.c_double)]
+    L.acgsolvercuda_solve_multi.argtypes = [P(acgsolvercuda), P(acgsymcsrmatrix), C.c_int, f64p, f64p, C.c_int,
+                                            C.c_double, C.c_double, C.c_int, P(acgb200_colstats)]
+    L.acgsolvercuda_spmm_mode.argtypes = [P(acgsolvercuda), C.c_int, C.c_int, f64p, C.c_void_p, f64p, P(C.c_double)]
     L.acgsolvercuda_info.argtypes = [P(acgsolvercuda), P(acgb200_info)]
     L.acgb200_set_option.argtypes = [C.c_char_p, C.c_int]
     L.acgb200_nccl_unique_id.argtypes = [C.c_void_p]
@@ -699,6 +708,47 @@ class SolverCuda:
         _check(lib().acgsolvercuda_spmv_mode(C.byref(self.c), int(mode), x, bp, y, int(path), C.byref(dot)),
                "acgsolvercuda_spmv_mode")
         return y, dot.value
+
+    def _block(self, M, name):
+        if not (isinstance(M, np.ndarray) and M.dtype == np.float64 and M.ndim == 2 and M.flags.c_contiguous):
+            raise ValueError(f"{name} must be a C-contiguous float64 array of shape (n, k)")
+        if M.shape[0] != self.A.c.nownedrows:
+            raise ValueError(f"{name} has shape {M.shape}: want ({self.A.c.nownedrows}, k)")
+        return M
+
+    def solve_multi(self, B, X, maxits=100, residualatol=0.0, residualrtol=0.0, warmup=0,
+                    raise_on_not_converged=False):
+        """acgsolvercuda_solve_multi: classic CG on the k columns of B at once, one pass over the matrix
+        per iteration for all of them; each column runs exactly the recurrence ``solvempi`` runs for it
+        alone.  B and X are C-contiguous float64 arrays of shape (n, k), 1 <= k <= 8; X holds the initial
+        guesses and is updated in place.  Returns (code, [per-column dict of niterations, converged,
+        bnrm2, r0nrm2, rnrm2])."""
+        B = self._block(B, "B")
+        X = self._block(X, "X")
+        if B.shape != X.shape:
+            raise ValueError(f"B {B.shape} and X {X.shape} differ")
+        k = B.shape[1]
+        st = (acgb200_colstats * k)()
+        code = lib().acgsolvercuda_solve_multi(C.byref(self.c), C.byref(self.A.c), k, B, X, int(maxits),
+                                               float(residualatol), float(residualrtol), int(warmup), st)
+        if code != ACG_SUCCESS and (raise_on_not_converged or code != ACG_ERR_NOT_CONVERGED):
+            raise AcgError(code, "acgsolvercuda_solve_multi", 0)
+        return code, [{n: getattr(s, n) for n, _ in acgb200_colstats._fields_} for s in st]
+
+    def spmm_mode(self, mode: int, X: np.ndarray, B: np.ndarray | None = None):
+        """The multi-vector product of solve_multi in one of the epilogue modes (acgsolvercuda_spmm_mode):
+        mode 0 Y = A X, 1 Y = A X with dots[j] = x_j.y_j, 2 Y = B - A X with dots[j] = y_j.y_j.
+        X, B: float64 (n, k).  Returns (Y, dots)."""
+        X = self._block(np.ascontiguousarray(X, np.float64), "X")
+        k = X.shape[1]
+        bp = None
+        if B is not None:
+            B = self._block(np.ascontiguousarray(B, np.float64), "B")
+            bp = B.ctypes.data_as(C.c_void_p)
+        Y = np.zeros_like(X)
+        dots = (C.c_double * k)()
+        _check(lib().acgsolvercuda_spmm_mode(C.byref(self.c), int(mode), k, X, bp, Y, dots), "acgsolvercuda_spmm_mode")
+        return Y, np.array(dots[:], np.float64)
 
     def info(self) -> dict:
         inf = acgb200_info()

@@ -164,6 +164,13 @@ struct priv {
     double last_spmv_ms;                /* profiled SpMV time of the last solve */
     double last_blas_ms;                /* profiled fused-update time of the last solve */
     int last_spmv_n;
+    int commsize;                       /* ranks of the communicator given to acgsolvercuda_init */
+    /* several right-hand sides (acgsolvercuda_solve_multi), made at the first multi-vector call */
+    struct acgb200_mstate *d_ms, *h_ms; /* per-column scalars on the device / pinned staging */
+    double *d_mx, *d_mb, *d_mr, *d_mp, *d_mt;   /* block vectors X, B, R, P, T: nowned x mk, interleaved */
+    int mk;                             /* their width */
+    int *d_ranges;                      /* [2 * nranges] row chunks outside the pattern slices */
+    int nranges, ranges_lanes, have_ranges;
 };
 
 /* The public struct has no room for private state (its layout is the
@@ -263,6 +270,8 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
         if (pv->redstream) cudaStreamDestroy(pv->redstream);
         if (pv->ev_red) cudaEventDestroy(pv->ev_red);
         cudaFree(pv->d_b); cudaFree(pv->d_x);
+        cudaFree(pv->d_ms); cudaFreeHost(pv->h_ms); cudaFree(pv->d_ranges);
+        cudaFree(pv->d_mx); cudaFree(pv->d_mb); cudaFree(pv->d_mr); cudaFree(pv->d_mp); cudaFree(pv->d_mt);
         if (pv->ev_ready) cudaEventDestroy(pv->ev_ready);
         if (pv->ev_halo) cudaEventDestroy(pv->ev_halo);
         for (int i = 0; i < 2; i++) if (pv->ev_poll[i]) cudaEventDestroy(pv->ev_poll[i]);
@@ -630,6 +639,7 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
         }
     }
 
+    pv->commsize = commsize;
     pv->nowned = A->nownedrows; pv->ninner = A->ninnerrows; pv->nborder = A->nborderrows;
     pv->nghost = A->nghostrows; pv->borderoff = A->borderrowoffset;
     pv->nvec = cg->r.num_nonzeros;
@@ -766,6 +776,7 @@ struct solvectx {
     int launches;
     int capturing;            /* inside cudaStreamBeginCapture: no profiling marks */
     int p2p;                  /* loop exchanges go through peer memory */
+    int mk;                   /* multi-vector loop: block width K (0: single vector) */
 };
 
 static int evpool_reserve(struct evpool *p, int n)
@@ -1004,7 +1015,7 @@ static double threshold(double atol, double rtol, double r0nrm2)
 static int graph_signature(const struct solvectx *c)
 {
     return 1 | (c->multi ? 2 : 0) | (c->p2p ? 4 : 0) | (c->pv->p2p.h_desc.fuse ? 8 : 0) | (cfg.pdl ? 16 : 0)
-           | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0);
+           | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0) | (c->mk << 8);
 }
 
 static int capture_pair(struct solvectx *c, int kind, int (*issue)(struct solvectx *, int))
@@ -1249,6 +1260,309 @@ int acgsolvercuda_solve(
     int errcode = 0;
     return acgsolvercuda_solvempi(cg, A, b, x, maxits, diffatol, diffrtol, residualatol, residualrtol,
                                   warmup, &null, 0, &errcode, NULL, NULL, 0);
+}
+
+/* ------------------------------------------------------------------------ */
+/* several right-hand sides: classic CG per column, one matrix pass for all  */
+/* ------------------------------------------------------------------------ */
+
+/* the multi-vector kernels are linked in (see ACGB200_MULTI_LAUNCHER, internal.h) */
+static int have_multi_kernels(void)
+{
+    return acgb200_spmm_launch && acgb200_cg_multi_update_r && acgb200_cg_multi_update_xp && acgb200_dot_multi;
+}
+
+static int block_width(int nrhs) { return nrhs <= 1 ? 1 : nrhs <= 2 ? 2 : nrhs <= 4 ? 4 : 8; }
+
+/* Rows the pattern slices do not cover, as chunks for spmm_rows_kernel: made once from the single-vector
+ * plan (its slices; every other row -- tile, merge, medium, long -- goes to the chunks).  Lanes per row
+ * from the mean length of those rows. */
+#define SPMM_CHUNK_LANES 128
+static int build_ranges(struct priv *pv, const struct acgsolvercuda *cg, int *errcode)
+{
+    if (pv->have_ranges) return ACG_SUCCESS;
+    const int n = pv->nowned, nsl = pv->plan.nslices;
+    unsigned char *cov = calloc((size_t) n + 1, 1);
+    int *rp = malloc(((size_t) n + 1) * sizeof(int));
+    struct acgb200_slice *sl = nsl > 0 ? malloc((size_t) nsl * sizeof(*sl)) : NULL;
+    int *rg = malloc(((size_t) n + 1) * 2 * sizeof(int));
+    if (!cov || !rp || (nsl > 0 && !sl) || !rg) { free(cov); free(rp); free(sl); free(rg); return ACG_ERR_ERRNO; }
+    cudaError_t e = cudaMemcpy(rp, cg->d_rowptr, ((size_t) n + 1) * sizeof(int), cudaMemcpyDeviceToHost);
+    if (!e && nsl > 0) e = cudaMemcpy(sl, pv->plan.d_slices, (size_t) nsl * sizeof(*sl), cudaMemcpyDeviceToHost);
+    if (e) { free(cov); free(rp); free(sl); free(rg); *errcode = (int) e; return ACG_ERR_CUDA; }
+    for (int s = 0; s < nsl; s++)
+        for (int r = sl[s].row0; r < sl[s].row0 + 32 && r < n; r++) cov[r] = 1;
+    int64_t urows = 0, unnz = 0;
+    for (int r = 0; r < n; r++) if (!cov[r]) { urows++; unnz += rp[r + 1] - rp[r]; }
+    const int lanes = urows > 0 && unnz > 12 * urows ? 8 : 1;
+    const int chunk = SPMM_CHUNK_LANES / lanes;      /* rows per chunk: four passes of a warp */
+    int nr = 0;
+    for (int r = 0; r < n;) {
+        if (cov[r]) { r++; continue; }
+        const int r0 = r;
+        while (r < n && !cov[r] && r - r0 < chunk) r++;
+        rg[2 * nr] = r0; rg[2 * nr + 1] = r; nr++;
+    }
+    if (nr > 0) {
+        e = cudaMalloc((void **) &pv->d_ranges, (size_t) nr * 2 * sizeof(int));
+        if (!e) e = cudaMemcpy(pv->d_ranges, rg, (size_t) nr * 2 * sizeof(int), cudaMemcpyHostToDevice);
+    }
+    free(cov); free(rp); free(sl); free(rg);
+    CU(e);
+    pv->nranges = nr; pv->ranges_lanes = lanes; pv->have_ranges = 1;
+    return ACG_SUCCESS;
+}
+
+/* per-column state and block vectors of width >= k, kept with the solver; a wider request replaces the
+ * blocks (and the captured multi-vector loop, whose pointers they were) */
+static int ensure_blocks(struct priv *pv, const struct acgsolvercuda *cg, int k, int *errcode)
+{
+    if (!pv->d_ms) {
+        CU(cudaMalloc((void **) &pv->d_ms, sizeof(*pv->d_ms)));
+        CU(cudaMemset(pv->d_ms, 0, sizeof(*pv->d_ms)));
+        CU(cudaMallocHost((void **) &pv->h_ms, sizeof(*pv->h_ms)));
+    }
+    OK(build_ranges(pv, cg, errcode));
+    if (pv->mk >= k) return ACG_SUCCESS;
+    double **blk[5] = { &pv->d_mx, &pv->d_mb, &pv->d_mr, &pv->d_mp, &pv->d_mt };
+    for (int i = 0; i < 5; i++) { cudaFree(*blk[i]); *blk[i] = NULL; }
+    if (pv->graph[2]) { cudaGraphExecDestroy(pv->graph[2]); pv->graph[2] = NULL; }
+    pv->mk = 0;
+    /* one spare row: the BLAS-1 kernels read pairs of entries */
+    const size_t bytes = ((size_t) pv->nowned + 1) * (size_t) k * sizeof(double);
+    for (int i = 0; i < 5; i++) {
+        CU(cudaMalloc((void **) blk[i], bytes));
+        CU(cudaMemset(*blk[i], 0, bytes));
+    }
+    pv->mk = k;
+    return ACG_SUCCESS;
+}
+
+/* n x nrhs row-major host array <-> n x k interleaved device block (padding columns zero) */
+static int upload_block_vec(struct priv *pv, double *dst, const double *src, int nrhs, int k, int *errcode)
+{
+    const size_t n = (size_t) pv->nowned;
+    if (nrhs == k) {
+        CU(cudaMemcpyAsync(dst, src, n * (size_t) k * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
+        CU(cudaStreamSynchronize(pv->stream));
+        return ACG_SUCCESS;
+    }
+    double *tmp = calloc(n * (size_t) k + 1, sizeof(double));
+    if (!tmp) return ACG_ERR_ERRNO;
+    for (size_t i = 0; i < n; i++) memcpy(tmp + i * (size_t) k, src + i * (size_t) nrhs, (size_t) nrhs * sizeof(double));
+    cudaError_t e = cudaMemcpyAsync(dst, tmp, n * (size_t) k * sizeof(double), cudaMemcpyHostToDevice, pv->stream);
+    if (!e) e = cudaStreamSynchronize(pv->stream);
+    free(tmp);
+    CU(e);
+    return ACG_SUCCESS;
+}
+
+static int download_block_vec(struct priv *pv, double *dst, const double *src, int nrhs, int k, int *errcode)
+{
+    const size_t n = (size_t) pv->nowned;
+    if (nrhs == k) {
+        CU(cudaMemcpyAsync(dst, src, n * (size_t) k * sizeof(double), cudaMemcpyDeviceToHost, pv->stream));
+        CU(cudaStreamSynchronize(pv->stream));
+        return ACG_SUCCESS;
+    }
+    double *tmp = malloc((n * (size_t) k + 1) * sizeof(double));
+    if (!tmp) return ACG_ERR_ERRNO;
+    cudaError_t e = cudaMemcpyAsync(tmp, src, n * (size_t) k * sizeof(double), cudaMemcpyDeviceToHost, pv->stream);
+    if (!e) e = cudaStreamSynchronize(pv->stream);
+    if (!e) for (size_t i = 0; i < n; i++) memcpy(dst + i * (size_t) nrhs, tmp + i * (size_t) k, (size_t) nrhs * sizeof(double));
+    free(tmp);
+    CU(e);
+    return ACG_SUCCESS;
+}
+
+static int push_mstate(struct solvectx *c, const struct acgb200_mstate *ms)
+{
+    int *errcode = c->errcode;
+    CU(cudaStreamSynchronize(c->pv->stream));
+    *c->pv->h_ms = *ms;
+    CU(cudaMemcpyAsync(c->pv->d_ms, c->pv->h_ms, sizeof(*ms), cudaMemcpyHostToDevice, c->pv->stream));
+    CU(cudaStreamSynchronize(c->pv->stream));
+    return ACG_SUCCESS;
+}
+
+static int pull_mstate(struct solvectx *c, struct acgb200_mstate *ms)
+{
+    int *errcode = c->errcode;
+    CU(cudaMemcpyAsync(c->pv->h_ms, c->pv->d_ms, sizeof(*ms), cudaMemcpyDeviceToHost, c->pv->stream));
+    CU(cudaStreamSynchronize(c->pv->stream));
+    *ms = *c->pv->h_ms;
+    return ACG_SUCCESS;
+}
+
+/* the multi-vector product of block x into block y (see struct acgb200_spmmargs) */
+static int apply_A_multi(struct solvectx *c, const double *x, double *y, const double *b, int mode, double *acc, int gated)
+{
+    struct acgsolvercuda *cg = c->cg;
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    struct acgb200_spmmargs a;
+    memset(&a, 0, sizeof(a));
+    a.plan = &pv->plan; a.k = c->mk;
+    a.nranges = pv->nranges; a.ranges = pv->d_ranges; a.lanes = pv->ranges_lanes;
+    a.rowptr = cg->d_rowptr; a.colidx = cg->d_colidx; a.a = cg->d_a;
+    a.x = x; a.y = y; a.b = b; a.acc = acc; a.mode = mode;
+    a.st = pv->d_st;
+    if (gated) { a.ctrl_in = &pv->d_st->ctrl[0]; a.ctrl_out = &pv->d_st->ctrl[1]; a.ms = pv->d_ms; }
+    prof_mark(c, &pv->gemv);
+    KL(acgb200_spmm_launch(&a, pv->stream));
+    prof_mark(c, &pv->gemv);
+    c->launches += (pv->plan.nslices > 0) + (pv->nranges > 0 || (gated && pv->plan.nslices == 0));
+    return ACG_SUCCESS;
+}
+
+/* one iteration of the K recurrences: T = A P (+ p_j.t_j), R -= alpha T (+ r_j.r_j), X += alpha P ; P = R + beta P */
+static int multi_iteration(struct solvectx *c, int k)
+{
+    struct priv *pv = c->pv;
+    struct acgb200_mstate *ms = pv->d_ms;
+    int *errcode = c->errcode;
+    const int s = k & 1, n = pv->nowned;
+    OK(apply_A_multi(c, pv->d_mp, pv->d_mt, NULL, SPMV_Y_AX_DOT, &ms->pap[s][0], 1));
+    prof_mark(c, &pv->blas);
+    KL(acgb200_cg_multi_update_r(n, c->mk, pv->d_st, ms, 1, 1, pv->d_mt, pv->d_mr, pv->stream));
+    KL(acgb200_cg_multi_update_xp(n, c->mk, pv->d_st, ms, 1, 0, pv->d_mr, pv->d_mp, c->d_x, pv->stream));
+    prof_mark(c, &pv->blas);
+    c->launches += 2;
+    return ACG_SUCCESS;
+}
+
+static void account_multi(struct acgsolvercuda *cg, const struct priv *pv, int nits, int k)
+{
+    /* per iteration: one pass over the matrix for K vectors, K columns of BLAS-1 */
+    const int64_t n = pv->nowned, nnz = pv->fnnz + pv->onnz, kk = k;
+    cg->ngemv += nits; cg->nflops += (int64_t) nits * 3 * nnz * kk;
+    cg->Bgemv += (int64_t) nits * (nnz * 12 + n * 4 + kk * n * 24);
+    cg->ndot += nits * kk; cg->nflops += (int64_t) nits * 2 * n * kk; cg->Bdot += (int64_t) nits * 16 * n * kk;
+    cg->nnrm2 += nits * kk; cg->nflops += (int64_t) nits * 2 * n * kk; cg->Bnrm2 += (int64_t) nits * 8 * n * kk;
+    cg->naxpy += 3 * (int64_t) nits * kk; cg->nflops += (int64_t) nits * 6 * n * kk; cg->Baxpy += (int64_t) nits * 48 * n * kk;
+}
+
+int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A,
+                              int nrhs, const double *B, double *X, int maxits, double residualatol, double residualrtol,
+                              int warmup, struct acgb200_colstats *stats)
+{
+    int errcode_ = 0, *errcode = &errcode_;
+    cfg_load();
+    struct priv *pv = priv_of(cg);
+    if (!pv) return ACG_ERR_INVALID_VALUE;
+    if (!have_multi_kernels() || pv->nghost > 0 || pv->commsize > 1 || (A && A->nghostrows > 0))
+        return ACG_ERR_NOT_SUPPORTED;      /* one GPU, whole matrix */
+    if (nrhs < 1 || nrhs > ACGB200_MAXK || !B || !X || maxits < 0) return ACG_ERR_INVALID_VALUE;
+    const int K = block_width(nrhs), n = pv->nowned;
+    OK(ensure_blocks(pv, cg, K, errcode));
+    struct solvectx c;
+    memset(&c, 0, sizeof(c));
+    c.cg = cg; c.pv = pv; c.errcode = errcode; c.mk = K;
+    c.d_b = pv->d_mb; c.d_x = pv->d_mx;
+    const double tb = wall();
+    OK(upload_block_vec(pv, pv->d_mb, B, nrhs, K, errcode));
+    OK(upload_block_vec(pv, pv->d_mx, X, nrhs, K, errcode));
+    pv->last_h2d_ms = 1e3 * (wall() - tb);
+    struct acgb200_devstate h;
+    struct acgb200_mstate m;
+
+    /* warm-up: `warmup` iterations of every column on state that is overwritten below; R stands in for X
+     * (as d_r does in acgsolvercuda_solvempi), so the initial guesses are untouched */
+    if (warmup > 0) {
+        memset(&m, 0, sizeof(m));
+        for (int j = 0; j < ACGB200_MAXK; j++) m.rr[0][j] = 1.0;
+        OK(push_mstate(&c, &m));
+        memset(&h, 0, sizeof(h));
+        h.maxits = warmup; h.ctrl[0].pad0 = (1 << K) - 1;
+        OK(push_state(&c, &h));
+        c.d_x = pv->d_mr;
+        for (int i = 0; i < warmup; i++) OK(multi_iteration(&c, i));
+        c.d_x = pv->d_mx;
+        KL(acgb200_dot_multi(n, K, pv->d_mb, &pv->d_ms->tmp[0], pv->stream));
+        CU(cudaStreamSynchronize(pv->stream));
+    }
+    if (cfg.profile) {
+        OK(evpool_reserve(&pv->gemv, 2 * (maxits + 2)));
+        OK(evpool_reserve(&pv->blas, 2 * (maxits + 2)));
+    }
+    pv->gemv.n = pv->blas.n = 0;
+
+    cg->nsolves++; cg->niterations = 0;
+    cg->bnrm2 = cg->r0nrm2 = cg->rnrm2 = cg->x0nrm2 = cg->dxnrm2 = INFINITY;
+    cg->maxits = maxits; cg->diffatol = 0; cg->diffrtol = 0;
+    cg->residualatol = residualatol; cg->residualrtol = residualrtol;
+    CU(cudaStreamSynchronize(pv->stream));
+    const double t0 = wall();
+    CU(cudaEventRecord(pv->ev_t0, pv->stream));
+    c.launches = 0;
+
+    /* ||b_j|| ; r0 = B - A X0 with (r0_j,r0_j) folded in ; P = R */
+    memset(&h, 0, sizeof(h));
+    OK(push_state(&c, &h));
+    memset(&m, 0, sizeof(m));
+    OK(push_mstate(&c, &m));
+    KL(acgb200_dot_multi(n, K, pv->d_mb, &pv->d_ms->tmp[0], pv->stream));
+    OK(apply_A_multi(&c, pv->d_mx, pv->d_mr, pv->d_mb, SPMV_R_B_AX, &pv->d_ms->rr[0][0], 0));
+    CU(cudaMemcpyAsync(pv->d_mp, pv->d_mr, (size_t) n * K * sizeof(double), cudaMemcpyDeviceToDevice, pv->stream));
+    OK(pull_mstate(&c, &m));
+    c.launches += 1;
+    double bb[ACGB200_MAXK], rr0[ACGB200_MAXK], tol[ACGB200_MAXK], rtol_scaled[ACGB200_MAXK];
+    unsigned mask = 0;
+    int poll = 0;
+    for (int j = 0; j < nrhs; j++) {
+        bb[j] = m.tmp[j]; rr0[j] = m.rr[0][j];
+        tol[j] = threshold(residualatol, residualrtol, sqrt(rr0[j]));
+        rtol_scaled[j] = residualrtol * sqrt(rr0[j]);
+        if (!(tol[j] > 0 && sqrt(rr0[j]) < tol[j])) mask |= 1u << j;       /* acg/cgcuda.c:836-842 per column */
+        if (tol[j] > 0) poll = 1;
+    }
+    int nits[ACGB200_MAXK], conv[ACGB200_MAXK];
+    double rr[ACGB200_MAXK];
+    for (int j = 0; j < nrhs; j++) { nits[j] = 0; conv[j] = !(mask >> j & 1u); rr[j] = rr0[j]; }
+    if (maxits > 0 && mask) {
+        memset(&m, 0, sizeof(m));
+        for (int j = 0; j < nrhs; j++) { m.tol[j] = tol[j]; m.rr[0][j] = rr0[j]; m.final_rr[j] = rr0[j]; }
+        OK(push_mstate(&c, &m));
+        memset(&h, 0, sizeof(h));
+        h.maxits = maxits; h.ctrl[0].pad0 = (int) mask;
+        OK(push_state(&c, &h));
+        OK(iterate(&c, maxits, poll, 2, multi_iteration));
+        OK(pull_state(&c, &h));
+        OK(pull_mstate(&c, &m));
+        cg->niterations = h.ctrl[0].iter;
+        for (int j = 0; j < nrhs; j++)
+            if (mask >> j & 1u) { nits[j] = m.nits[j]; conv[j] = m.conv[j]; rr[j] = m.final_rr[j]; }
+    }
+    cg->ntotaliterations += cg->niterations;
+    CU(cudaEventRecord(pv->ev_t1, pv->stream));
+    CU(cudaEventSynchronize(pv->ev_t1));
+    cg->tsolve += wall() - t0;
+    { float ms = 0; if (cudaEventElapsedTime(&ms, pv->ev_t0, pv->ev_t1) == cudaSuccess) pv->last_solve_ms = ms; }
+    account_multi(cg, pv, cg->niterations, K);
+    cg->ngemv++; cg->ncopy += 1; cg->nnrm2 += 2 * nrhs;
+    pv->last_launches = c.launches;
+    if (cfg.profile) {
+        pv->last_spmv_ms = evpool_sum_ms(&pv->gemv); pv->last_spmv_n = pv->gemv.n / 2;
+        pv->last_blas_ms = evpool_sum_ms(&pv->blas);
+        cg->tgemv += 1e-3 * pv->last_spmv_ms;
+        cg->taxpy += 1e-3 * pv->last_blas_ms;
+    }
+    double sb = 0, sr0 = 0, sr = 0;
+    int status = ACG_SUCCESS;
+    for (int j = 0; j < nrhs; j++) {
+        sb += bb[j]; sr0 += rr0[j]; sr += rr[j];
+        if (!conv[j] && !(residualatol == 0 && rtol_scaled[j] == 0)) status = ACG_ERR_NOT_CONVERGED;   /* :1099-1107 per column */
+        if (stats) {
+            stats[j].niterations = nits[j]; stats[j].converged = conv[j];
+            stats[j].bnrm2 = sqrt(bb[j]); stats[j].r0nrm2 = sqrt(rr0[j]); stats[j].rnrm2 = sqrt(rr[j]);
+        }
+    }
+    cg->bnrm2 = sqrt(sb); cg->r0nrm2 = sqrt(sr0); cg->rnrm2 = sqrt(sr);
+    const double te = wall();
+    OK(download_block_vec(pv, X, pv->d_mx, nrhs, K, errcode));
+    pv->last_d2h_ms = 1e3 * (wall() - te);
+    CU(cudaGetLastError());
+    return status;
 }
 
 /* ------------------------------------------------------------------------ */
@@ -1746,6 +2060,37 @@ int acgsolvercuda_spmv_mode(struct acgsolvercuda *cg, int mode, const double *x,
     return ACG_SUCCESS;
 }
 
+/* The multi-vector product of acgsolvercuda_solve_multi in any of the three epilogue modes, for
+ * nrhs columns (padded to the block width K as the solver pads them): X, B (mode 2) and Y are host
+ * arrays of nowned x nrhs doubles, row-major; dots[j] gets column j's fused dot.  Y is poisoned on
+ * the device first, so a row no kernel writes reads NaN. */
+int acgsolvercuda_spmm_mode(struct acgsolvercuda *cg, int mode, int nrhs, const double *X, const double *B, double *Y,
+                            double *dots)
+{
+    int errcode_ = 0, *errcode = &errcode_;
+    struct priv *pv = priv_of(cg);
+    if (!pv) return ACG_ERR_INVALID_VALUE;
+    if (!have_multi_kernels() || pv->nghost > 0 || pv->commsize > 1) return ACG_ERR_NOT_SUPPORTED;
+    if (nrhs < 1 || nrhs > ACGB200_MAXK || !X || !Y) return ACG_ERR_INVALID_VALUE;
+    if (mode != SPMV_Y_AX && mode != SPMV_Y_AX_DOT && mode != SPMV_R_B_AX) return ACG_ERR_INVALID_VALUE;
+    if (mode == SPMV_R_B_AX && !B) return ACG_ERR_INVALID_VALUE;
+    const int K = block_width(nrhs), n = pv->nowned;
+    OK(ensure_blocks(pv, cg, K, errcode));
+    OK(upload_block_vec(pv, pv->d_mp, X, nrhs, K, errcode));
+    if (mode == SPMV_R_B_AX) OK(upload_block_vec(pv, pv->d_mb, B, nrhs, K, errcode));
+    CU(cudaMemsetAsync(pv->d_mt, 0xff, (size_t) n * K * sizeof(double), pv->stream));
+    CU(cudaMemsetAsync(&pv->d_ms->tmp[0], 0, sizeof(pv->d_ms->tmp), pv->stream));
+    struct solvectx c;
+    memset(&c, 0, sizeof(c));
+    c.cg = cg; c.pv = pv; c.errcode = errcode; c.mk = K;
+    OK(apply_A_multi(&c, pv->d_mp, pv->d_mt, mode == SPMV_R_B_AX ? pv->d_mb : NULL, mode, &pv->d_ms->tmp[0], 0));
+    OK(download_block_vec(pv, Y, pv->d_mt, nrhs, K, errcode));
+    double h[ACGB200_MAXK];
+    CU(cudaMemcpy(h, &pv->d_ms->tmp[0], sizeof(h), cudaMemcpyDeviceToHost));
+    if (dots) for (int j = 0; j < nrhs; j++) dots[j] = h[j];
+    return ACG_SUCCESS;
+}
+
 int acgsolvercuda_spmv_ghost(struct acgsolvercuda *cg, const double *x, double *y, int path, double *dot)
 {
     return acgsolvercuda_spmv_mode(cg, SPMV_Y_AX_DOT, x, NULL, y, path, dot);
@@ -1776,5 +2121,7 @@ int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info
     info->spmv_merge_threads = pv->plan.merge_threads; info->spmv_merge_grid = pv->plan.merge_grid;
     info->spmv_merge_stages = pv->plan.merge_stages;
     info->spmv_min_bytes = acgb200_spmv_min_bytes(&pv->plan);
+    info->spmv_slice_value_bytes = pv->plan.nslices > 0 ? pv->plan.sval_blocks * 32 * (int64_t) sizeof(double) : 0;
+    info->spmv_slice_nnz = pv->plan.nslices > 0 ? pv->plan.slice_nnz : 0;
     return ACG_SUCCESS;
 }

@@ -321,6 +321,62 @@ int acgb200_expand_upload(const struct acgsymcsrmatrix *A, double eps, int rp_pa
                           struct acgb200_expanded *out, cudaStream_t stream, int *errcode);
 void acgb200_expanded_free(struct acgb200_expanded *x);
 
+/* ------------------------------------------------------------------------
+ * Several right-hand sides (acgsolvercuda_solve_multi): K independent classic
+ * CG recurrences that share every pass over the matrix.  Block vectors hold K
+ * columns interleaved, entry (row, j) at row*K + j, K in {1,2,4,8}.  Columns
+ * beyond the caller's count are padding, inactive from the start.  The
+ * active-column mask travels with the control word (ctrl.pad0, bit j), so it
+ * follows the same ring as the iteration index.
+ * ------------------------------------------------------------------------ */
+#define ACGB200_MAXK 8
+
+struct acgb200_mstate {
+    double rr[2][ACGB200_MAXK];      /* (r_j,r_j) of iteration k in slot k&1 */
+    double pap[2][ACGB200_MAXK];     /* (p_j,A p_j) of iteration k in slot k&1 */
+    double tol[ACGB200_MAXK];        /* stop column j when ||r_j|| < tol[j] (0: never) */
+    double final_rr[ACGB200_MAXK];   /* (r_j,r_j) of the column's last iterate */
+    double tmp[ACGB200_MAXK];        /* set-up reductions */
+    int nits[ACGB200_MAXK];          /* iterations the column ran */
+    int conv[ACGB200_MAXK];          /* 1: the column met its tolerance */
+};
+
+struct acgb200_spmmargs {
+    const struct acgb200_spmvplan *plan;  /* pattern slices of the single-vector plan */
+    int k;                                /* block width K */
+    int nranges;                          /* row chunks outside the slices, spmm_rows_kernel */
+    const int *ranges;                    /* [2 * nranges]: first row, one past the last row */
+    int lanes;                            /* lanes per row of spmm_rows_kernel: 1 or 8 */
+    const int *rowptr, *colidx;
+    const double *a;
+    const double *x;                      /* n x K */
+    double *y;                            /* n x K */
+    const double *b;                      /* n x K, SPMV_R_B_AX */
+    double *acc;                          /* [K] fused per-column dots (modes 1, 2); may be NULL */
+    int mode;                             /* SPMV_Y_AX, SPMV_Y_AX_DOT or SPMV_R_B_AX */
+    const struct acgb200_ctrl *ctrl_in;   /* may be NULL: unconditional */
+    struct acgb200_ctrl *ctrl_out;
+    const struct acgb200_devstate *st;    /* maxits of the gate */
+    struct acgb200_mstate *ms;            /* housekeeping: the first kernel zeroes ms->rr[s^1] (may be NULL) */
+};
+/* The host code (cgcuda.c) references the four multi-vector launchers weakly: a host build that carries the
+ * single-vector kernels only -- the host-logic test build of tests/hostsim -- still loads, and
+ * acgsolvercuda_solve_multi / acgsolvercuda_spmm_mode return ACG_ERR_NOT_SUPPORTED there (no other path
+ * runs instead).  libacgb200.so always defines them (kernels.cu). */
+#if defined(__CUDACC__)
+#define ACGB200_MULTI_LAUNCHER
+#else
+#define ACGB200_MULTI_LAUNCHER __attribute__((weak))
+#endif
+ACGB200_MULTI_LAUNCHER int acgb200_spmm_launch(const struct acgb200_spmmargs *a, cudaStream_t stream);
+/* classic CG updates with per-column alpha_j, beta_j; columns outside the incoming mask are left alone */
+ACGB200_MULTI_LAUNCHER int acgb200_cg_multi_update_r(int n, int k, struct acgb200_devstate *st, struct acgb200_mstate *ms, int cin, int cout,
+                              const double *t, double *r, cudaStream_t stream);
+ACGB200_MULTI_LAUNCHER int acgb200_cg_multi_update_xp(int n, int k, struct acgb200_devstate *st, struct acgb200_mstate *ms, int cin, int cout,
+                               const double *r, double *p, double *x, cudaStream_t stream);
+/* acc[j] += sum_i x[i*k + j]^2 */
+ACGB200_MULTI_LAUNCHER int acgb200_dot_multi(int n, int k, const double *x, double *acc, cudaStream_t stream);
+
 /* setup-time helpers */
 int acgb200_dot(int n, const double *x, const double *y, double *acc, cudaStream_t stream); /* acc += x.y */
 int acgb200_dot2(int n, const double *r, const double *w, double *acc2, cudaStream_t stream); /* acc2[0]+=r.r, acc2[1]+=w.r */

@@ -1318,6 +1318,373 @@ __global__ void scatter_kernel(int n, const double *__restrict__ src, double *__
 }
 
 /* ------------------------------------------------------------------------ */
+/* several right-hand sides: block vectors of K interleaved columns          */
+/* ------------------------------------------------------------------------ */
+
+/* the K entries of one row of a block vector through the read-only path: vector loads of two
+ * doubles (16-byte aligned, as row*K is even for K >= 2), issued back to back like ld_x */
+template <int K>
+__device__ __forceinline__ void ld_xk(double (&v)[K], const double *p)
+{
+    if constexpr (K == 1) {
+        v[0] = ld_x(p);
+    } else {
+#pragma unroll
+        for (int h = 0; h < K / 2; h++)
+            asm volatile("ld.global.nc.v2.f64 {%0, %1}, [%2];" : "=d"(v[2 * h]), "=d"(v[2 * h + 1]) : "l"(p + 2 * h));
+    }
+}
+
+/* one finished row of K columns: y = A x (mode 0, 1, with dot_j += x_j y_j in mode 1) or
+ * y = b - A x with dot_j += y_j^2 (mode 2) */
+template <int K>
+__device__ __forceinline__ void spmm_row_epilogue(int row, const double (&sum)[K], int mode, const double *x, double *y,
+                                                  const double *b, double (&dot)[K])
+{
+    const size_t o = (size_t) row * K;
+    if (mode == SPMV_R_B_AX) {
+#pragma unroll
+        for (int j = 0; j < K; j++) {
+            const double v = b[o + j] - sum[j];
+            y[o + j] = v;
+            dot[j] = fma(v, v, dot[j]);
+        }
+    } else {
+#pragma unroll
+        for (int j = 0; j < K; j++) y[o + j] = sum[j];
+        if (mode == SPMV_Y_AX_DOT) {
+#pragma unroll
+            for (int j = 0; j < K; j++) dot[j] = fma(__ldg(x + o + j), sum[j], dot[j]);
+        }
+    }
+}
+
+/* per-column sums over the CTA, then one atomicAdd per non-zero column sum; `red` holds
+ * blockDim/32 * K doubles */
+template <int K>
+__device__ __forceinline__ void block_sum_k_add(double (&v)[K], double *red, double *acc)
+{
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31, nw = (blockDim.x + 31) >> 5;
+#pragma unroll
+    for (int j = 0; j < K; j++) v[j] = warp_sum(v[j]);
+    if (l == 0) {
+#pragma unroll
+        for (int j = 0; j < K; j++) red[w * K + j] = v[j];
+    }
+    __syncthreads();
+    if ((int) threadIdx.x < K) {
+        double s = 0.0;
+        for (int i = 0; i < nw; i++) s += red[i * K + threadIdx.x];
+        if (s != 0.0) atomicAdd(acc + threadIdx.x, s);
+    }
+}
+
+/* the first kernel of a gated multi-vector product forwards the control word and clears the (r,r)
+ * accumulators the update behind it adds into (nothing reads them during the product) */
+__device__ __forceinline__ void spmm_housekeeping(const acgb200_ctrl *cin, acgb200_ctrl *cout, const Gate &g,
+                                                  acgb200_mstate *ms)
+{
+    if (blockIdx.x == 0 && threadIdx.x == 0 && cin && cout) {
+        *cout = *cin;
+        if (g.active && ms) {
+#pragma unroll
+            for (int j = 0; j < ACGB200_MAXK; j++) ms->rr[(g.iter & 1) ^ 1][j] = 0.0;
+        }
+    }
+}
+
+struct SpmmParams {
+    const acgb200_slice *slices;
+    int nslices;
+    const double *sval;
+    const unsigned short *patid;
+    const int *spatoff;
+    int npat, lpad;
+    const int2 *ranges;
+    int nranges;
+    const int *rowptr;
+    const int *colidx;
+    const double *a;
+    const double *x;
+    double *y;
+    const double *b;
+    double *acc;
+    int mode;
+    const acgb200_ctrl *ctrl_in;
+    acgb200_ctrl *ctrl_out;        /* NULL: another kernel of the product forwards the word */
+    const acgb200_devstate *st;
+    acgb200_mstate *ms;
+};
+
+/*
+ * The slice kernel for K columns: one warp per slice, one row per lane, the same slice-major values,
+ * evict-first streaming loads and offset table as spmv_slices_kernel.  Each value is loaded once and
+ * fused into K accumulators; the x entries of a slot are one vector gather of K doubles.  UB slots are
+ * in flight per batch (UB * K gathers).  Every column is summed in slot (CSR) order, as the
+ * single-vector kernel sums its one column.  EXC: lanes of exception rows take their columns from the
+ * CSR index array; slots past a row's end hold the value 0 and gather x[row].
+ */
+template <int UB, int T, bool EXC, int K>
+__global__ void __launch_bounds__(T)
+spmm_slices_kernel(const SpmmParams P)
+{
+    extern __shared__ __align__(16) int spat_s[];
+    __shared__ double red[T / 32 * K];
+    const int tid = threadIdx.x;
+    pdl_prologue();
+    const Gate gate = gate_read(P.ctrl_in, P.st);
+    spmm_housekeeping(P.ctrl_in, P.ctrl_out, gate, P.ms);
+    if (!gate.active) return;
+    for (int i = tid; i < P.npat * P.lpad; i += T) spat_s[i] = P.spatoff[i];
+    __syncthreads();
+
+    const uint64_t pol = l2_policy_evict_first();
+    const int lane = tid & 31;
+    const int warp = (blockIdx.x * T + tid) >> 5;
+    const int nwarps = (gridDim.x * T) >> 5;
+    double dot[K];
+#pragma unroll
+    for (int j = 0; j < K; j++) dot[j] = 0.0;
+    for (int s = warp; s < P.nslices; s += nwarps) {
+        const int4 sl = __ldg(reinterpret_cast<const int4 *>(P.slices) + s);     /* row0, nrows, len, vblk */
+        const int row = sl.x + lane;
+        const int pid = P.patid[row];
+        const bool exc = EXC && pid == (int) ACGB200_NOPATTERN;
+        const int *offs = spat_s + (exc ? 0 : pid) * P.lpad;
+        const double *v = P.sval + ((size_t) sl.w << 5) + lane;
+        const int L = sl.z;
+        int kb = 0, len = 0;
+        if (EXC && exc) { kb = P.rowptr[row]; len = P.rowptr[row + 1] - kb; }
+        double sum[K];
+#pragma unroll
+        for (int j = 0; j < K; j++) sum[j] = 0.0;
+        int e = 0;
+        /* full batches: straight-line code, all UB value loads and UB*K gathers issued before the first FMA */
+        for (; e + UB <= L; e += UB) {
+            double vv[UB], xv[UB][K];
+#pragma unroll
+            for (int u = 0; u < UB; u++) vv[u] = ld_stream(v + (size_t) (e + u) * 32, pol);
+#pragma unroll
+            for (int u = 0; u < UB; u++) {
+                int col = row + offs[e + u];
+                if (EXC && exc) col = e + u < len ? __ldg(P.colidx + kb + e + u) : row;
+                ld_xk<K>(xv[u], P.x + (size_t) col * K);
+            }
+#pragma unroll
+            for (int u = 0; u < UB; u++) {
+#pragma unroll
+                for (int j = 0; j < K; j++) sum[j] = fma(vv[u], xv[u][j], sum[j]);
+            }
+        }
+        /* last, partial batch slot by slot */
+        for (; e < L; e++) {
+            double xv[K];
+            int col = row + offs[e];
+            if (EXC && exc) col = e < len ? __ldg(P.colidx + kb + e) : row;
+            const double vv = ld_stream(v + (size_t) e * 32, pol);
+            ld_xk<K>(xv, P.x + (size_t) col * K);
+#pragma unroll
+            for (int j = 0; j < K; j++) sum[j] = fma(vv, xv[j], sum[j]);
+        }
+        spmm_row_epilogue<K>(row, sum, P.mode, P.x, P.y, P.b, dot);
+    }
+    if (P.acc) block_sum_k_add<K>(dot, red, P.acc);
+}
+
+/*
+ * Every row outside the pattern slices (tile, merge, medium and long rows of the single-vector plan),
+ * plain CSR: a warp per chunk of rows (P.ranges), G lanes per row, each column index and value read
+ * once per nonzero and fused into K accumulators.  With G > 1 a row's lanes are combined by a fixed
+ * shuffle tree.  Long rows are correct here, not fast.
+ */
+template <int G, int K>
+__global__ void __launch_bounds__(256)
+spmm_rows_kernel(const SpmmParams P)
+{
+    __shared__ double red[256 / 32 * K];
+    pdl_prologue();
+    const Gate gate = gate_read(P.ctrl_in, P.st);
+    spmm_housekeeping(P.ctrl_in, P.ctrl_out, gate, P.ms);
+    if (!gate.active) return;
+    const int lane = threadIdx.x & 31;
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int nwarps = (gridDim.x * blockDim.x) >> 5;
+    double dot[K];
+#pragma unroll
+    for (int j = 0; j < K; j++) dot[j] = 0.0;
+    for (int c = warp; c < P.nranges; c += nwarps) {
+        const int2 rg = P.ranges[c];
+        for (int base = rg.x; base < rg.y; base += 32 / G) {
+            const int row = base + lane / G;
+            double sum[K];
+#pragma unroll
+            for (int j = 0; j < K; j++) sum[j] = 0.0;
+            if (row < rg.y) {
+                const int ke = P.rowptr[row + 1];
+#pragma unroll 1
+                for (int k = P.rowptr[row] + lane % G; k < ke; k += G) {
+                    double xv[K];
+                    const double av = __ldg(P.a + k);
+                    ld_xk<K>(xv, P.x + (size_t) __ldg(P.colidx + k) * K);
+#pragma unroll
+                    for (int j = 0; j < K; j++) sum[j] = fma(av, xv[j], sum[j]);
+                }
+            }
+            if (G > 1) {
+#pragma unroll
+                for (int j = 0; j < K; j++) sum[j] = group_sum<G>(sum[j]);
+            }
+            if (row < rg.y && lane % G == 0) spmm_row_epilogue<K>(row, sum, P.mode, P.x, P.y, P.b, dot);
+        }
+    }
+    if (P.acc) block_sum_k_add<K>(dot, red, P.acc);
+}
+
+/* A thread of the grid-stride BLAS-1 loops over a block vector reads pairs of entries (double2) and the
+ * stride is a multiple of K, so its columns never change: c0 = 2g mod K and c0 + 1 (both 0 for K = 1).
+ * Per-column sums: lanes 2l mod K hold the same pair, so an xor-shuffle over offsets >= K/2 leaves the
+ * warp's sums of columns 2l, 2l+1 in lane l < K/2; then one atomicAdd per column and CTA (of the
+ * columns in `mask`). */
+template <int K>
+__device__ __forceinline__ void colpair_sum_add(double a0, double a1, double *red, double *acc, unsigned mask)
+{
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31, nw = (blockDim.x + 31) >> 5;
+    if constexpr (K == 1) {
+        const double v = block_sum(a0 + a1, red);
+        if (threadIdx.x == 0 && (mask & 1u)) atomicAdd(acc, v);
+    } else {
+#pragma unroll
+        for (int o = 16; o >= K / 2; o >>= 1) {
+            a0 += __shfl_xor_sync(0xffffffffu, a0, o);
+            a1 += __shfl_xor_sync(0xffffffffu, a1, o);
+        }
+        if (l < K / 2) { red[w * K + 2 * l] = a0; red[w * K + 2 * l + 1] = a1; }
+        __syncthreads();
+        if ((int) threadIdx.x < K && (mask >> threadIdx.x & 1u)) {
+            double s = 0.0;
+            for (int i = 0; i < nw; i++) s += red[i * K + threadIdx.x];
+            atomicAdd(acc + threadIdx.x, s);
+        }
+    }
+}
+
+/* R_j -= alpha_j T_j with alpha_j = (r_j,r_j)/(p_j,Ap_j), and the new (r_j,r_j), for the active columns */
+template <int K>
+__global__ void __launch_bounds__(BLAS1_THREADS)
+cg_multi_update_r_kernel(int n, acgb200_devstate *st, acgb200_mstate *ms, int cin, int cout,
+                         const double *__restrict__ t, double *__restrict__ r)
+{
+    __shared__ double red[BLAS1_THREADS / 32 * (K > 1 ? K : 1)];
+    pdl_prologue();
+    const Gate g = gate_read(&st->ctrl[cin], st);
+    if (cin != cout && blockIdx.x == 0 && threadIdx.x == 0) st->ctrl[cout] = st->ctrl[cin];
+    if (!g.active) return;
+    const unsigned mask = (unsigned) st->ctrl[cin].pad0;
+    const int s = g.iter & 1;
+    const int gtid = blockIdx.x * blockDim.x + threadIdx.x, gstride = gridDim.x * blockDim.x;
+    const int c0 = (2 * gtid) & (K - 1), c1 = K == 1 ? 0 : c0 + 1;
+    const bool act0 = mask >> c0 & 1u, act1 = mask >> c1 & 1u;
+    const double al0 = act0 ? ms->rr[s][c0] / ms->pap[s][c0] : 0.0;
+    const double al1 = act1 ? ms->rr[s][c1] / ms->pap[s][c1] : 0.0;
+    double acc0 = 0.0, acc1 = 0.0;
+    const long long nk = (long long) n * K, n2 = nk >> 1;
+    const double2 *t2 = reinterpret_cast<const double2 *>(t);
+    double2 *r2 = reinterpret_cast<double2 *>(r);
+    for (long long i = gtid; i < n2; i += gstride) {
+        const double2 tv = t2[i];
+        double2 rv = r2[i];
+        if (act0) rv.x = fma(-al0, tv.x, rv.x);
+        if (act1) rv.y = fma(-al1, tv.y, rv.y);
+        r2[i] = rv;
+        acc0 = fma(rv.x, rv.x, acc0);
+        acc1 = fma(rv.y, rv.y, acc1);
+    }
+    if ((nk & 1) && blockIdx.x == 0 && threadIdx.x == 0 && act0) {     /* K = 1, n odd */
+        const double rv = fma(-al0, t[nk - 1], r[nk - 1]);
+        r[nk - 1] = rv;
+        acc0 = fma(rv, rv, acc0);
+    }
+    colpair_sum_add<K>(acc0, acc1, red, &ms->rr[s ^ 1][0], mask);
+}
+
+/* X_j += alpha_j P_j ; P_j = R_j + beta_j P_j for the active columns.  Block 0 decides each column's
+ * convergence for the next iteration: a column that meets its tolerance leaves the mask (its x is the
+ * iterate just formed), its iteration count and final (r,r) are recorded; with no column left the
+ * control word is marked done. */
+template <int K>
+__global__ void __launch_bounds__(BLAS1_THREADS)
+cg_multi_update_xp_kernel(int n, acgb200_devstate *st, acgb200_mstate *ms, int cin, int cout,
+                          const double *__restrict__ r, double *__restrict__ p, double *__restrict__ x)
+{
+    pdl_prologue();
+    const Gate g = gate_read(&st->ctrl[cin], st);
+    const int s = g.iter & 1;
+    const unsigned mask = (unsigned) st->ctrl[cin].pad0;
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        acgb200_ctrl c = st->ctrl[cin];
+        if (g.active) {
+            unsigned next = mask;
+            c.iter = g.iter + 1;
+            for (int j = 0; j < K; j++) {
+                if (!(mask >> j & 1u)) continue;
+                const double rrn = ms->rr[s ^ 1][j];
+                ms->nits[j] = g.iter + 1;
+                ms->final_rr[j] = rrn;
+                /* acg/cgcuda.c:1008-1012 per column: ||r_j|| < tol_j, strictly */
+                if (ms->tol[j] > 0.0 && sqrt(rrn) < ms->tol[j]) { next &= ~(1u << j); ms->conv[j] = 1; }
+            }
+            for (int j = 0; j < ACGB200_MAXK; j++) ms->pap[s ^ 1][j] = 0.0;     /* accumulators of the next product */
+            c.pad0 = (int) next;
+            if (next == 0) c.done = 1;
+        }
+        st->ctrl[cout] = c;
+    }
+    if (!g.active) return;
+    const int gtid = blockIdx.x * blockDim.x + threadIdx.x, gstride = gridDim.x * blockDim.x;
+    const int c0 = (2 * gtid) & (K - 1), c1 = K == 1 ? 0 : c0 + 1;
+    const bool act0 = mask >> c0 & 1u, act1 = mask >> c1 & 1u;
+    const double al0 = act0 ? ms->rr[s][c0] / ms->pap[s][c0] : 0.0, be0 = act0 ? ms->rr[s ^ 1][c0] / ms->rr[s][c0] : 0.0;
+    const double al1 = act1 ? ms->rr[s][c1] / ms->pap[s][c1] : 0.0, be1 = act1 ? ms->rr[s ^ 1][c1] / ms->rr[s][c1] : 0.0;
+    const long long nk = (long long) n * K, n2 = nk >> 1;
+    const double2 *r2 = reinterpret_cast<const double2 *>(r);
+    double2 *p2 = reinterpret_cast<double2 *>(p);
+    double2 *x2 = reinterpret_cast<double2 *>(x);
+    for (long long i = gtid; i < n2; i += gstride) {
+        const double2 rv = r2[i];
+        double2 pv = p2[i];
+        double2 xv = x2[i];
+        if (act0) { xv.x = fma(al0, pv.x, xv.x); pv.x = fma(be0, pv.x, rv.x); }
+        if (act1) { xv.y = fma(al1, pv.y, xv.y); pv.y = fma(be1, pv.y, rv.y); }
+        x2[i] = xv;
+        p2[i] = pv;
+    }
+    if ((nk & 1) && blockIdx.x == 0 && threadIdx.x == 0 && act0) {
+        const double pv = p[nk - 1];
+        x[nk - 1] = fma(al0, pv, x[nk - 1]);
+        p[nk - 1] = fma(be0, pv, r[nk - 1]);
+    }
+}
+
+/* acc[j] += sum_i x[i*K + j]^2 (set-up: ||b_j||^2) */
+template <int K>
+__global__ void __launch_bounds__(BLAS1_THREADS)
+dot_multi_kernel(int n, const double *__restrict__ x, double *acc)
+{
+    __shared__ double red[BLAS1_THREADS / 32 * (K > 1 ? K : 1)];
+    const int gtid = blockIdx.x * blockDim.x + threadIdx.x, gstride = gridDim.x * blockDim.x;
+    const long long nk = (long long) n * K, n2 = nk >> 1;
+    const double2 *x2 = reinterpret_cast<const double2 *>(x);
+    double a0 = 0.0, a1 = 0.0;
+    for (long long i = gtid; i < n2; i += gstride) {
+        const double2 v = x2[i];
+        a0 = fma(v.x, v.x, a0);
+        a1 = fma(v.y, v.y, a1);
+    }
+    if ((nk & 1) && blockIdx.x == 0 && threadIdx.x == 0) a0 = fma(x[nk - 1], x[nk - 1], a0);
+    colpair_sum_add<K>(a0, a1, red, acc, (1u << K) - 1u);
+}
+
+/* ------------------------------------------------------------------------ */
 /* host-side launchers (C linkage)                                           */
 /* ------------------------------------------------------------------------ */
 
@@ -1635,6 +2002,121 @@ extern "C" int acgb200_dot2(int n, const double *r, const double *w, double *acc
     static int occ = 0;
     dot2_kernel<<<blas1_grid(n, (const void *) dot2_kernel, &occ), BLAS1_THREADS, 0, stream>>>(n, r, w, acc2);
     return (int) cudaGetLastError();
+}
+
+/* ---- several right-hand sides -------------------------------------------------------------- */
+
+typedef void (*spmm_fn)(const SpmmParams);
+
+/* slots per batch of the multi-vector slice kernel: UB * K gathers in flight per lane (16 for K >= 2) */
+#define SPMM_SLICE_UB(K) ((K) == 1 ? 8 : 16 / (K) < 2 ? 2 : 16 / (K))
+#define SPMM_SLICE_T 128
+#define SPMM_ROWS_T 256
+
+static spmm_fn spmm_slice_variant(int K, int EXC)
+{
+#define XS(k) if (K == k) return EXC ? spmm_slices_kernel<SPMM_SLICE_UB(k), SPMM_SLICE_T, true, k> \
+                                     : spmm_slices_kernel<SPMM_SLICE_UB(k), SPMM_SLICE_T, false, k>;
+    XS(1) XS(2) XS(4) XS(8)
+#undef XS
+    return NULL;
+}
+
+static spmm_fn spmm_rows_variant(int G, int K)
+{
+#define XR(k) if (K == k) return G == 8 ? spmm_rows_kernel<8, k> : G == 1 ? spmm_rows_kernel<1, k> : NULL;
+    XR(1) XR(2) XR(4) XR(8)
+#undef XR
+    return NULL;
+}
+
+/* resident CTAs per SM of a kernel (cached per function) */
+static int spmm_per_sm(const void *fn, int threads, size_t smem)
+{
+    static const void *fns[64];
+    static int val[64], nfn = 0;
+    for (int i = 0; i < nfn; i++) if (fns[i] == fn) return val[i];
+    int per = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, fn, threads, smem) != cudaSuccess || per < 1) per = 1;
+    if (nfn < 64) { fns[nfn] = fn; val[nfn] = per; nfn++; }
+    return per;
+}
+
+extern "C" int acgb200_spmm_launch(const acgb200_spmmargs *a, cudaStream_t stream)
+{
+    const acgb200_spmvplan *pl = a->plan;
+    SpmmParams P;
+    memset(&P, 0, sizeof(P));
+    P.slices = pl->d_slices; P.nslices = pl->nslices; P.sval = pl->d_sval;
+    P.patid = pl->d_spatid; P.spatoff = pl->d_spatoff; P.npat = pl->slice_npat; P.lpad = pl->slice_lpad;
+    P.ranges = reinterpret_cast<const int2 *>(a->ranges); P.nranges = a->nranges;
+    P.rowptr = a->rowptr; P.colidx = a->colidx; P.a = a->a;
+    P.x = a->x; P.y = a->y; P.b = a->b; P.acc = a->acc; P.mode = a->mode;
+    P.ctrl_in = a->ctrl_in; P.st = a->st; P.ms = a->ms;
+    /* the first kernel forwards the control word; the second reads the same incoming word (only the
+     * iteration's last kernel rewrites it) */
+    bool forwarded = false;
+    if (pl->nslices > 0) {
+        const spmm_fn fn = spmm_slice_variant(a->k, pl->slice_exc > 0);
+        if (!fn) return (int) cudaErrorInvalidConfiguration;
+        const size_t smem = (size_t) ((pl->slice_npat * pl->slice_lpad + 3) & ~3) * sizeof(int);
+        if (smem > 48 * 1024) {
+            const cudaError_t e = cudaFuncSetAttribute((const void *) fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+            if (e) return (int) e;
+        }
+        long long grid = (long long) acgb200_num_sms() * spmm_per_sm((const void *) fn, SPMM_SLICE_T, smem);
+        const long long need = ((long long) pl->nslices * 32 + SPMM_SLICE_T - 1) / SPMM_SLICE_T;
+        if (grid > need) grid = need;
+        P.ctrl_out = a->ctrl_out;
+        forwarded = true;
+        const cudaError_t le = launch_chain(fn, (int) (grid < 1 ? 1 : grid), SPMM_SLICE_T, smem, stream, P);
+        if (le) return (int) le;
+    }
+    if (a->nranges > 0 || (a->ctrl_in && !forwarded)) {
+        const spmm_fn fn = spmm_rows_variant(a->lanes, a->k);
+        if (!fn) return (int) cudaErrorInvalidConfiguration;
+        long long grid = (long long) acgb200_num_sms() * spmm_per_sm((const void *) fn, SPMM_ROWS_T, 0);
+        const long long need = ((long long) a->nranges + SPMM_ROWS_T / 32 - 1) / (SPMM_ROWS_T / 32);
+        if (grid > need) grid = need;
+        P.ctrl_out = forwarded ? NULL : a->ctrl_out;
+        P.ms = forwarded ? NULL : a->ms;
+        const cudaError_t le = launch_chain(fn, (int) (grid < 1 ? 1 : grid), SPMM_ROWS_T, 0, stream, P);
+        if (le) return (int) le;
+    }
+    return (int) cudaGetLastError();
+}
+
+/* the BLAS-1 grid of a block vector: as blas1_grid over its n*K entries */
+#define MULTI_K_DISPATCH(k, call) \
+    ((k) == 1 ? (call(1)) : (k) == 2 ? (call(2)) : (k) == 4 ? (call(4)) : (k) == 8 ? (call(8)) : cudaErrorInvalidValue)
+
+extern "C" int acgb200_cg_multi_update_r(int n, int k, acgb200_devstate *st, acgb200_mstate *ms, int cin, int cout,
+                                         const double *t, double *r, cudaStream_t stream)
+{
+    static int occ[9];
+#define CALL(K) launch_chain(cg_multi_update_r_kernel<K>, blas1_grid(n * K, (const void *) cg_multi_update_r_kernel<K>, &occ[K]), \
+                             BLAS1_THREADS, 0, stream, n, st, ms, cin, cout, t, r)
+    return (int) MULTI_K_DISPATCH(k, CALL);
+#undef CALL
+}
+
+extern "C" int acgb200_cg_multi_update_xp(int n, int k, acgb200_devstate *st, acgb200_mstate *ms, int cin, int cout,
+                                          const double *r, double *p, double *x, cudaStream_t stream)
+{
+    static int occ[9];
+#define CALL(K) launch_chain(cg_multi_update_xp_kernel<K>, blas1_grid(n * K, (const void *) cg_multi_update_xp_kernel<K>, &occ[K]), \
+                             BLAS1_THREADS, 0, stream, n, st, ms, cin, cout, r, p, x)
+    return (int) MULTI_K_DISPATCH(k, CALL);
+#undef CALL
+}
+
+extern "C" int acgb200_dot_multi(int n, int k, const double *x, double *acc, cudaStream_t stream)
+{
+    static int occ[9];
+#define CALL(K) (dot_multi_kernel<K><<<blas1_grid(n * K, (const void *) dot_multi_kernel<K>, &occ[K]), BLAS1_THREADS, 0, stream>>>(n, x, acc), \
+                 cudaGetLastError())
+    return (int) MULTI_K_DISPATCH(k, CALL);
+#undef CALL
 }
 
 extern "C" int acgb200_gather(int n, double *dst, const double *src, const int *idx, cudaStream_t stream)

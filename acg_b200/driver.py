@@ -42,6 +42,9 @@ def parse_args(argv=None):
                          "(mtxpartition output, as the reference's --partition=FILE)")
     ap.add_argument("--manufactured-solution", action="store_true",
                     help="random unit x*, b = A x*, report ||x - x*|| (cuda/acg-cuda.c:1969-1979, :2376-2385)")
+    ap.add_argument("--nrhs", type=int, default=None,
+                    help="solve K (1-8) seeded right-hand sides at once: classic CG per column, one pass over the matrix per "
+                         "iteration for all of them (acgsolvercuda_solve_multi; one process only)")
     ap.add_argument("--seed", type=int, default=1)
     ap.add_argument("--output-comm-matrix", metavar="PATH", help="write the halo send-count matrix (cuda/acg-cuda.c:1713-1775)")
     ap.add_argument("--output-solution", metavar="PATH", help="write x as a Matrix Market vector (text)")
@@ -97,6 +100,47 @@ def local_rhs(args, A, n):
     return b, xloc[:no]
 
 
+def multi_rhs(args, A, n):
+    """--nrhs K: K seeded right-hand sides, or with --manufactured-solution K seeded unit-norm solutions
+    X* and B = A X* (column j from seed + j).  Returns (B, X*) as (n, K) arrays; X* is None otherwise."""
+    k = args.nrhs
+    if not args.manufactured_solution:
+        B = np.stack([np.random.default_rng(args.seed + j).uniform(-1.0, 1.0, n) for j in range(k)], axis=1)
+        return np.ascontiguousarray(B), None
+    Xs = np.stack([np.random.default_rng(args.seed + j).uniform(-1.0, 1.0, n) for j in range(k)], axis=1)
+    Xs /= np.linalg.norm(Xs, axis=0)
+    import scipy.sparse as sp
+    rp = A.frowptr[:n + 1]
+    F = sp.csr_matrix((A.fa[:rp[n]], A.fcolidx[:rp[n]] - A.c.rowidxbase, rp), shape=(n, n))
+    return np.ascontiguousarray(F @ Xs), np.ascontiguousarray(Xs)
+
+
+def solve_multi(args, A, cg, n, log):
+    """The --nrhs run: one solve_multi call, the solver report, then iterations and residual per column
+    (and the initial and final error norms with --manufactured-solution)."""
+    B, Xs = multi_rhs(args, A, n)
+    X = np.zeros_like(B)
+    code, cols = cg.solve_multi(B, X, maxits=args.max_iterations, residualatol=args.residual_atol,
+                                residualrtol=args.residual_rtol, warmup=args.warmup)
+    log(cg.report())
+    log(f"right-hand sides: {args.nrhs}")
+    for j, c in enumerate(cols):
+        line = (f"  column {j}: iterations {c['niterations']} converged {c['converged']} "
+                f"residual 2-norm {c['rnrm2']:.15g} relative {c['rnrm2'] / c['r0nrm2'] if c['r0nrm2'] else 0.0:.3e}")
+        if Xs is not None:
+            line += (f" initial error 2-norm {np.linalg.norm(Xs[:, j]):.15g}"
+                     f" error 2-norm {np.linalg.norm(X[:, j] - Xs[:, j]):.15g}")
+        log(line)
+    if args.output_solution:
+        from . import mtxio
+        for j in range(args.nrhs):
+            root, ext = os.path.splitext(args.output_solution)
+            mtxio.write_vector(f"{root}.{j}{ext}", X[:, j], binary=False)
+    if code != 0:
+        log(f"acg_b200.driver: solver returned {code} (not converged)")
+    return code
+
+
 def main(argv=None):
     args = parse_args(argv)
     # torchrun exports OMP_NUM_THREADS=1 unless the caller set it; the ingest and the full-storage
@@ -109,6 +153,13 @@ def main(argv=None):
     from . import dist as abdist, mtxio
     from .api import SolverCuda, SymCsrMatrix, mtx_info
 
+    if args.nrhs is not None:
+        if not 1 <= args.nrhs <= 8:
+            raise SystemExit("--nrhs must be between 1 and 8")
+        if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            raise SystemExit("--nrhs runs in one process (one GPU, the whole matrix)")
+        if args.solver != "acg":
+            raise SystemExit("--nrhs solves with classic CG (--solver acg)")
     rank, world, _local = abdist.init_process(backend="gloo")
     log = (lambda *a: print(*a, file=sys.stderr, flush=True)) if rank == 0 else (lambda *a: None)
     if world > 1 and not args.binary:
@@ -148,6 +199,11 @@ def main(argv=None):
         raise SystemExit("acg_b200.driver: no CUDA device (the solver has no CPU path; --dry-run stops before it)")
     comm = abdist.nccl_comm(rank, world)
     cg = SolverCuda(A, comm)
+    if args.nrhs is not None:
+        code = solve_multi(args, A, cg, n, log)
+        cg.free()
+        comm.destroy()
+        return 0 if code == 0 else 1
     b = A.vector(); x = A.vector()
     bo, xstar = local_rhs(args, A, n)
     no = A.c.nownedrows

@@ -50,6 +50,33 @@ ACG_API int acgsolvercuda_spmv_ghost(struct acgsolvercuda *cg, const double *x, 
 ACG_API int acgsolvercuda_spmv_mode(struct acgsolvercuda *cg, int mode, const double *x, const double *b, double *y,
                                     int path, double *dot);
 
+/* Several right-hand sides of one operator in one pass over the matrix per iteration: nrhs (1..8)
+ * independent classic CG recurrences, column j exactly the recurrence acgsolvercuda_solvempi runs for
+ * that column alone (its own alpha_j, beta_j, threshold(atol, rtol, ||r0_j||), strict ||r_j|| < tol_j
+ * test; a column that meets it stops, its x frozen at that iterate).  Not block CG: the columns share
+ * the matrix reads, nothing else.  B and X are host arrays of nownedrows x nrhs doubles, row-major
+ * (entry (i, j) at i*nrhs + j); X is the initial guess on entry and the solution on return.  One GPU,
+ * unpartitioned matrix: ghost rows or a communicator of more than one rank give ACG_ERR_NOT_SUPPORTED,
+ * nrhs outside [1, 8] ACG_ERR_INVALID_VALUE.  Returns ACG_ERR_NOT_CONVERGED if a column with a non-zero
+ * tolerance did not converge.  In *cg: niterations is the iterations the loop ran (the maximum over the
+ * columns), bnrm2 / r0nrm2 / rnrm2 the Frobenius norms over the columns; stats (may be NULL, nrhs
+ * entries) gets each column's own figures. */
+struct acgb200_colstats {
+    int niterations;            /* iterations this column ran */
+    int converged;              /* 1: it met its tolerance (at r0 or later) */
+    double bnrm2, r0nrm2, rnrm2;
+};
+ACG_API int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A,
+                                      int nrhs, const double *B, double *X, int maxits, double residualatol,
+                                      double residualrtol, int warmup, struct acgb200_colstats *stats);
+
+/* The multi-vector product of acgsolvercuda_solve_multi in epilogue mode 0 (Y = A X), 1 (Y = A X,
+ * dots[j] = x_j.y_j) or 2 (Y = B - A X, dots[j] = y_j.y_j); X, B (mode 2, else may be NULL), Y host
+ * arrays of nownedrows x nrhs doubles, row-major; dots (may be NULL) nrhs entries.  Y is poisoned on
+ * the device first, so a row no kernel writes comes back NaN.  For tests against exact products. */
+ACG_API int acgsolvercuda_spmm_mode(struct acgsolvercuda *cg, int mode, int nrhs, const double *X, const double *B,
+                                    double *Y, double *dots);
+
 struct acgb200_info {
     int spmv_lanes_per_row, spmv_rows_cap, spmv_nnz_cap, spmv_stages;
     int spmv_ntiles, spmv_nlong, spmv_grid, spmv_smem_bytes;
@@ -76,6 +103,8 @@ struct acgb200_info {
     int spmv_threads, spmv_unroll;              /* shape of the tile kernel (with spmv_lanes_per_row) */
     int spmv_slice_threads;                     /* CTA size of the slice kernel (with spmv_slice_ub) */
     int spmv_merge_threads, spmv_merge_grid, spmv_merge_stages;    /* shape and grid of the merge-path kernel */
+    int64_t spmv_slice_value_bytes;             /* slice-major values of the pattern slices, padding included */
+    int64_t spmv_slice_nnz;                     /* nonzeros those slices cover (without padding) */
 };
 ACG_API int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info);
 
