@@ -159,7 +159,7 @@ EXPORTS = [
     "acgsolvercuda_init_constants", "acgsolvercuda_alpha", "acgsolvercuda_beta", "acgsolvercuda_daxpy_alpha",
     "acgsolvercuda_daxpy_minus_alpha", "acgsolvercuda_daypx_beta", "acgsolvercuda_pipelined_daxpy_fused",
     "acgsolvercuda_fwrite",
-    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_solve_multi", "acgsolvercuda_spmm_mode", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
+    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_solve_multi", "acgsolvercuda_spmm_mode", "acgsolvercuda_solve_shifted", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
     "acgb200_nccl_unique_id", "acgb200_comm_init_rank", "acgb200_comm_destroy",
     "acgb200_host_register", "acgb200_host_unregister", "acgb200_spmv_plan_host", "acgb200_spmv_plan_host2", "acgb200_slices_host", "acgb200_merge_plan_host", "acgb200_p2p_inverse_map", "acgb200_patterns_host", "acgb200_stencil_part",
     "acgb200_mtx_info", "acgb200_mtx_read", "acgb200_mtx_read_part", "acgb200_comm_matrix_row", "acgb200_partition_rows_grid", "acgb200_grid_factors", "acgb200_rmat_spd",
@@ -241,6 +241,8 @@ def lib() -> C.CDLL:
     L.acgsolvercuda_solve_multi.argtypes = [P(acgsolvercuda), P(acgsymcsrmatrix), C.c_int, f64p, f64p, C.c_int,
                                             C.c_double, C.c_double, C.c_int, P(acgb200_colstats)]
     L.acgsolvercuda_spmm_mode.argtypes = [P(acgsolvercuda), C.c_int, C.c_int, f64p, C.c_void_p, f64p, P(C.c_double)]
+    L.acgsolvercuda_solve_shifted.argtypes = [P(acgsolvercuda), P(acgsymcsrmatrix), C.c_int, f64p, f64p, f64p, C.c_int,
+                                              C.c_double, C.c_double, C.c_int, P(acgb200_colstats)]
     L.acgsolvercuda_info.argtypes = [P(acgsolvercuda), P(acgb200_info)]
     L.acgb200_set_option.argtypes = [C.c_char_p, C.c_int]
     L.acgb200_nccl_unique_id.argtypes = [C.c_void_p]
@@ -734,6 +736,29 @@ class SolverCuda:
         if code != ACG_SUCCESS and (raise_on_not_converged or code != ACG_ERR_NOT_CONVERGED):
             raise AcgError(code, "acgsolvercuda_solve_multi", 0)
         return code, [{n: getattr(s, n) for n, _ in acgb200_colstats._fields_} for s in st]
+
+    def solve_shifted(self, b, shifts, maxits=100, residualatol=0.0, residualrtol=0.0, warmup=0,
+                      raise_on_not_converged=False):
+        """acgsolvercuda_solve_shifted: (A + shifts[j] I) x_j = b for 1 <= S <= 8 finite shifts >= 0 in one
+        Krylov space (multi-shift CG): one product per iteration for all shifts.  Every system starts from
+        x0 = 0; shift j stops by the rule ``solvempi`` applies to that system alone.  b: float64 array of
+        the owned rows.  Returns (code, X of shape (n, S), [per-shift dict of niterations, converged,
+        bnrm2, r0nrm2, rnrm2])."""
+        b = np.ascontiguousarray(b, np.float64)
+        if b.shape != (self.A.c.nownedrows,):
+            raise ValueError(f"b has shape {b.shape}: want ({self.A.c.nownedrows},)")
+        shifts = np.ascontiguousarray(np.atleast_1d(np.asarray(shifts, np.float64)))
+        if shifts.ndim != 1:
+            raise ValueError(f"shifts must be one-dimensional, not of shape {shifts.shape}")
+        S = len(shifts)
+        X = self._block(np.zeros((self.A.c.nownedrows, max(S, 1)), np.float64), "X")
+        st = (acgb200_colstats * max(S, 1))()
+        code = lib().acgsolvercuda_solve_shifted(C.byref(self.c), C.byref(self.A.c), S,
+                                                 shifts if S else np.zeros(1), b, X, int(maxits),
+                                                 float(residualatol), float(residualrtol), int(warmup), st)
+        if code != ACG_SUCCESS and (raise_on_not_converged or code != ACG_ERR_NOT_CONVERGED):
+            raise AcgError(code, "acgsolvercuda_solve_shifted", 0)
+        return code, X, [{n: getattr(s, n) for n, _ in acgb200_colstats._fields_} for s in st[:S]]
 
     def spmm_mode(self, mode: int, X: np.ndarray, B: np.ndarray | None = None):
         """The multi-vector product of solve_multi in one of the epilogue modes (acgsolvercuda_spmm_mode):

@@ -153,9 +153,10 @@ struct priv {
     struct acgcomm redcomm;             /* private duplicate of the caller's communicator for reductions */
     int have_redcomm;
     double *d_b, *d_x;                  /* right-hand side / solution on the device, kept between solves */
-    cudaGraphExec_t graph[3];           /* [0] classic, [1] pipelined ([2] spare): two iterations each (parity 0 then 1) */
-    int graph_sig[3];                   /* loop configuration each cached graph was captured with (graph_signature) */
-    int graph_launches[3];              /* kernel/NCCL launches inside one replay */
+    cudaGraphExec_t graph[4];           /* [0] classic, [1] pipelined, [2] several right-hand sides, [3] shifted
+                                         * systems: two iterations each (parity 0 then 1) */
+    int graph_sig[4];                   /* loop configuration each cached graph was captured with (graph_signature) */
+    int graph_launches[4];              /* kernel/NCCL launches inside one replay */
     double last_h2d_ms, last_d2h_ms;    /* host time spent before / after the solve window */
     cudaEvent_t ev_t0, ev_t1;           /* device-side bracket of the solve window */
     double last_solve_ms;
@@ -171,6 +172,8 @@ struct priv {
     int mk;                             /* their width */
     int *d_ranges;                      /* [2 * nranges] row chunks outside the pattern slices */
     int nranges, ranges_lanes, have_ranges;
+    /* shifted systems (acgsolvercuda_solve_shifted): per-shift scalars; the vectors are the blocks above */
+    struct acgb200_sstate *d_ss, *h_ss;
 };
 
 /* The public struct has no room for private state (its layout is the
@@ -259,7 +262,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
             pv->p2p.window = NULL;
         }
         if (pv->have_redcomm && pv->redcomm.ncclcomm) ncclCommDestroy(pv->redcomm.ncclcomm);
-        for (int i = 0; i < 3; i++) if (pv->graph[i]) cudaGraphExecDestroy(pv->graph[i]);
+        for (int i = 0; i < 4; i++) if (pv->graph[i]) cudaGraphExecDestroy(pv->graph[i]);
         cudaFree(pv->plan.d_tiles); cudaFree(pv->plan.d_longrows); cudaFree(pv->plan.d_long_scratch); cudaFree(pv->plan.d_medrows);
         cudaFree(pv->plan.d_slices); cudaFree(pv->plan.d_sval); cudaFree(pv->plan.d_spatoff); cudaFree(pv->plan.d_spatid);
         cudaFree(pv->plan.d_mtiles); cudaFree(pv->plan.d_msplit); cudaFree(pv->plan.d_mpart);
@@ -271,6 +274,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
         if (pv->ev_red) cudaEventDestroy(pv->ev_red);
         cudaFree(pv->d_b); cudaFree(pv->d_x);
         cudaFree(pv->d_ms); cudaFreeHost(pv->h_ms); cudaFree(pv->d_ranges);
+        cudaFree(pv->d_ss); cudaFreeHost(pv->h_ss);
         cudaFree(pv->d_mx); cudaFree(pv->d_mb); cudaFree(pv->d_mr); cudaFree(pv->d_mp); cudaFree(pv->d_mt);
         if (pv->ev_ready) cudaEventDestroy(pv->ev_ready);
         if (pv->ev_halo) cudaEventDestroy(pv->ev_halo);
@@ -777,6 +781,7 @@ struct solvectx {
     int capturing;            /* inside cudaStreamBeginCapture: no profiling marks */
     int p2p;                  /* loop exchanges go through peer memory */
     int mk;                   /* multi-vector loop: block width K (0: single vector) */
+    int shifted;              /* shifted-systems loop (acgsolvercuda_solve_shifted) */
 };
 
 static int evpool_reserve(struct evpool *p, int n)
@@ -1015,7 +1020,7 @@ static double threshold(double atol, double rtol, double r0nrm2)
 static int graph_signature(const struct solvectx *c)
 {
     return 1 | (c->multi ? 2 : 0) | (c->p2p ? 4 : 0) | (c->pv->p2p.h_desc.fuse ? 8 : 0) | (cfg.pdl ? 16 : 0)
-           | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0) | (c->mk << 8);
+           | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0) | (c->shifted ? 128 : 0) | (c->mk << 8);
 }
 
 static int capture_pair(struct solvectx *c, int kind, int (*issue)(struct solvectx *, int))
@@ -1326,7 +1331,7 @@ static int ensure_blocks(struct priv *pv, const struct acgsolvercuda *cg, int k,
     if (pv->mk >= k) return ACG_SUCCESS;
     double **blk[5] = { &pv->d_mx, &pv->d_mb, &pv->d_mr, &pv->d_mp, &pv->d_mt };
     for (int i = 0; i < 5; i++) { cudaFree(*blk[i]); *blk[i] = NULL; }
-    if (pv->graph[2]) { cudaGraphExecDestroy(pv->graph[2]); pv->graph[2] = NULL; }
+    for (int i = 2; i < 4; i++) if (pv->graph[i]) { cudaGraphExecDestroy(pv->graph[i]); pv->graph[i] = NULL; }
     pv->mk = 0;
     /* one spare row: the BLAS-1 kernels read pairs of entries */
     const size_t bytes = ((size_t) pv->nowned + 1) * (size_t) k * sizeof(double);
@@ -1560,6 +1565,197 @@ int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acgsymcsrma
     cg->bnrm2 = sqrt(sb); cg->r0nrm2 = sqrt(sr0); cg->rnrm2 = sqrt(sr);
     const double te = wall();
     OK(download_block_vec(pv, X, pv->d_mx, nrhs, K, errcode));
+    pv->last_d2h_ms = 1e3 * (wall() - te);
+    CU(cudaGetLastError());
+    return status;
+}
+
+/* ------------------------------------------------------------------------ */
+/* shifted systems: one seed CG on A drives every (A + sigma_j I) x_j = b    */
+/* ------------------------------------------------------------------------ */
+
+/* the shift kernels are linked in (see ACGB200_MULTI_LAUNCHER, internal.h) */
+static int have_shift_kernels(void)
+{
+    return have_multi_kernels() && acgb200_shift_setup && acgb200_cg_shift_update;
+}
+
+static int push_sstate(struct solvectx *c, const struct acgb200_sstate *ss)
+{
+    int *errcode = c->errcode;
+    CU(cudaStreamSynchronize(c->pv->stream));
+    *c->pv->h_ss = *ss;
+    CU(cudaMemcpyAsync(c->pv->d_ss, c->pv->h_ss, sizeof(*ss), cudaMemcpyHostToDevice, c->pv->stream));
+    CU(cudaStreamSynchronize(c->pv->stream));
+    return ACG_SUCCESS;
+}
+
+static int pull_sstate(struct solvectx *c, struct acgb200_sstate *ss)
+{
+    int *errcode = c->errcode;
+    CU(cudaMemcpyAsync(c->pv->h_ss, c->pv->d_ss, sizeof(*ss), cudaMemcpyDeviceToHost, c->pv->stream));
+    CU(cudaStreamSynchronize(c->pv->stream));
+    *ss = *c->pv->h_ss;
+    return ACG_SUCCESS;
+}
+
+/* the state of iteration 0: zeta_0 = zeta_{-1} = 1, alpha_{-1} = 1, beta_{-1} = 0 */
+static void sstate_init(struct acgb200_sstate *ss, int nshifts, const double *shifts, double tol, double r0nrm2)
+{
+    memset(ss, 0, sizeof(*ss));
+    for (int j = 0; j < ACGB200_MAXK; j++) { ss->zeta[0][j] = 1.0; ss->zeta_prev[0][j] = 1.0; }
+    ss->ab_prev[0][0] = 1.0; ss->ab_prev[0][1] = 0.0;
+    for (int j = 0; j < nshifts; j++) { ss->sigma[j] = shifts[j]; ss->tol[j] = tol; ss->final_rnrm2[j] = r0nrm2; }
+}
+
+/* one seed iteration and the shift updates: t = A p (+ p.t), r -= alpha t (+ r.r), then
+ * p = r + beta p and X_j += alpha_j P_j ; P_j = zeta_j r + beta_j P_j */
+static int shifted_iteration(struct solvectx *c, int k)
+{
+    struct acgsolvercuda *cg = c->cg;
+    struct priv *pv = c->pv;
+    struct acgb200_devstate *st = pv->d_st;
+    int *errcode = c->errcode;
+    const int s = k & 1, n = pv->nowned;
+    OK(apply_A(c, cg->d_p, cg->d_p, cg->d_t, NULL, SPMV_Y_AX_DOT, &st->pap_loc[s], 1, 1, 0, 0));
+    prof_mark(c, &pv->blas);
+    KL(acgb200_cg_update_r(n, st, 1, 1, 0, NULL, cg->d_t, cg->d_r, pv->stream));
+    KL(acgb200_cg_shift_update(n, c->mk, st, pv->d_ss, 1, 0, cg->d_r, cg->d_p, c->d_x, pv->d_mp, pv->stream));
+    prof_mark(c, &pv->blas);
+    c->launches += 2;
+    return ACG_SUCCESS;
+}
+
+static void account_shifted(struct acgsolvercuda *cg, const struct priv *pv, int nits, int nshifts)
+{
+    /* per iteration: the classic product, r -= alpha t with (r,r), p = r + beta p, and per shift
+     * x_j += alpha_j p_j ; p_j = zeta_j r + beta_j p_j (x_j, p_j read and written: 32 B per row) */
+    const int64_t n = pv->nowned, nnz = pv->fnnz + pv->onnz, s = nshifts;
+    const int64_t bgemv = nnz * 12 + n * 16 + (int64_t) pv->nvec * 8;
+    cg->ngemv += nits; cg->nflops += (int64_t) nits * 3 * nnz; cg->Bgemv += (int64_t) nits * bgemv;
+    cg->ndot += nits; cg->nflops += (int64_t) nits * 2 * n; cg->Bdot += (int64_t) nits * 16 * n;
+    cg->nnrm2 += nits; cg->nflops += (int64_t) nits * 2 * n; cg->Bnrm2 += (int64_t) nits * 8 * n;
+    cg->naxpy += (int64_t) nits * (2 + 2 * s); cg->nflops += (int64_t) nits * (4 + 5 * s) * n;
+    cg->Baxpy += (int64_t) nits * (48 + 32 * s) * n;
+}
+
+int acgsolvercuda_solve_shifted(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A,
+                                int nshifts, const double *shifts, const double *b, double *X,
+                                int maxits, double residualatol, double residualrtol, int warmup,
+                                struct acgb200_colstats *stats)
+{
+    int errcode_ = 0, *errcode = &errcode_;
+    cfg_load();
+    struct priv *pv = priv_of(cg);
+    if (!pv) return ACG_ERR_INVALID_VALUE;
+    if (!have_shift_kernels() || pv->nghost > 0 || pv->commsize > 1 || (A && A->nghostrows > 0))
+        return ACG_ERR_NOT_SUPPORTED;      /* one GPU, whole matrix */
+    if (nshifts < 1 || nshifts > ACGB200_MAXK || !shifts || !b || !X || maxits < 0) return ACG_ERR_INVALID_VALUE;
+    for (int j = 0; j < nshifts; j++) if (!(isfinite(shifts[j]) && shifts[j] >= 0)) return ACG_ERR_INVALID_VALUE;
+    const int K = block_width(nshifts), n = pv->nowned;
+    OK(ensure_blocks(pv, cg, K, errcode));
+    if (!pv->d_ss) {
+        CU(cudaMalloc((void **) &pv->d_ss, sizeof(*pv->d_ss)));
+        CU(cudaMallocHost((void **) &pv->h_ss, sizeof(*pv->h_ss)));
+    }
+    struct solvectx c;
+    memset(&c, 0, sizeof(c));
+    c.cg = cg; c.pv = pv; c.errcode = errcode; c.mk = K; c.shifted = 1;
+    /* b lives in the first n entries of the B block, which this loop does not otherwise use */
+    double *const d_b = pv->d_mb;
+    c.d_b = d_b; c.d_x = pv->d_mx;
+    const double tb = wall();
+    CU(cudaMemcpyAsync(d_b, b, (size_t) n * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
+    CU(cudaStreamSynchronize(pv->stream));
+    pv->last_h2d_ms = 1e3 * (wall() - tb);
+    struct acgb200_devstate h;
+    struct acgb200_sstate ss;
+    const unsigned all = (1u << nshifts) - 1u;
+
+    /* warm-up: `warmup` iterations from the real set-up on state that is overwritten below; the R block
+     * stands in for X, so X is untouched */
+    if (warmup > 0) {
+        KL(acgb200_shift_setup(n, K, d_b, cg->d_r, cg->d_p, pv->d_mr, pv->d_mp, pv->stream));
+        sstate_init(&ss, nshifts, shifts, 0.0, 1.0);
+        OK(push_sstate(&c, &ss));
+        memset(&h, 0, sizeof(h));
+        h.maxits = warmup; h.rr_loc[0] = h.rr[0] = 1.0; h.ctrl[0].pad0 = (int) all;
+        OK(push_state(&c, &h));
+        c.d_x = pv->d_mr;
+        for (int i = 0; i < warmup; i++) OK(shifted_iteration(&c, i));
+        c.d_x = pv->d_mx;
+        CU(cudaStreamSynchronize(pv->stream));
+    }
+    if (cfg.profile) {
+        OK(evpool_reserve(&pv->gemv, 2 * (maxits + 2)));
+        OK(evpool_reserve(&pv->blas, 2 * (maxits + 2)));
+    }
+    pv->gemv.n = pv->blas.n = 0;
+
+    cg->nsolves++; cg->niterations = 0;
+    cg->bnrm2 = cg->r0nrm2 = cg->rnrm2 = cg->x0nrm2 = cg->dxnrm2 = INFINITY;
+    cg->maxits = maxits; cg->diffatol = 0; cg->diffrtol = 0;
+    cg->residualatol = residualatol; cg->residualrtol = residualrtol;
+    CU(cudaStreamSynchronize(pv->stream));
+    const double t0 = wall();
+    CU(cudaEventRecord(pv->ev_t0, pv->stream));
+    c.launches = 0;
+
+    /* r0 = p0 = b (x0 = 0 for every shift), X = 0, P_j = b ; ||b|| */
+    memset(&h, 0, sizeof(h));
+    OK(push_state(&c, &h));
+    KL(acgb200_shift_setup(n, K, d_b, cg->d_r, cg->d_p, pv->d_mx, pv->d_mp, pv->stream));
+    KL(acgb200_dot(n, d_b, d_b, &pv->d_st->tmp_loc[0], pv->stream));
+    double bb = 0;
+    OK(reduce_to_host(&c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &bb));
+    c.launches += 2;
+    const double bnrm2 = sqrt(bb);
+    const double tol = threshold(residualatol, residualrtol, bnrm2);
+    const double rtol_scaled = residualrtol * bnrm2;
+    /* every shifted system starts from r0 = b, so all meet the test at r0 or none does */
+    const unsigned mask = tol > 0 && bnrm2 < tol ? 0u : all;
+    int nits[ACGB200_MAXK], conv[ACGB200_MAXK];
+    double rn[ACGB200_MAXK];
+    for (int j = 0; j < nshifts; j++) { nits[j] = 0; conv[j] = !(mask >> j & 1u); rn[j] = bnrm2; }
+    if (maxits > 0 && mask) {
+        sstate_init(&ss, nshifts, shifts, tol, bnrm2);
+        OK(push_sstate(&c, &ss));
+        memset(&h, 0, sizeof(h));
+        h.maxits = maxits; h.rr_loc[0] = h.rr[0] = bb; h.ctrl[0].pad0 = (int) mask;
+        OK(push_state(&c, &h));
+        OK(iterate(&c, maxits, tol > 0, 3, shifted_iteration));
+        OK(pull_state(&c, &h));
+        OK(pull_sstate(&c, &ss));
+        cg->niterations = h.ctrl[0].iter;
+        for (int j = 0; j < nshifts; j++) { nits[j] = ss.nits[j]; conv[j] = ss.conv[j]; rn[j] = ss.final_rnrm2[j]; }
+    }
+    cg->ntotaliterations += cg->niterations;
+    CU(cudaEventRecord(pv->ev_t1, pv->stream));
+    CU(cudaEventSynchronize(pv->ev_t1));
+    cg->tsolve += wall() - t0;
+    { float ms = 0; if (cudaEventElapsedTime(&ms, pv->ev_t0, pv->ev_t1) == cudaSuccess) pv->last_solve_ms = ms; }
+    account_shifted(cg, pv, cg->niterations, nshifts);
+    cg->ncopy += 2; cg->nnrm2++;
+    pv->last_launches = c.launches;
+    if (cfg.profile) {
+        pv->last_spmv_ms = evpool_sum_ms(&pv->gemv); pv->last_spmv_n = pv->gemv.n / 2;
+        pv->last_blas_ms = evpool_sum_ms(&pv->blas);
+        cg->tgemv += 1e-3 * pv->last_spmv_ms;
+        cg->taxpy += 1e-3 * pv->last_blas_ms;
+    }
+    double sr = 0;
+    int status = ACG_SUCCESS;
+    for (int j = 0; j < nshifts; j++) {
+        sr += rn[j] * rn[j];
+        if (!conv[j] && !(residualatol == 0 && rtol_scaled == 0)) status = ACG_ERR_NOT_CONVERGED;   /* :1099-1107 per shift */
+        if (stats) {
+            stats[j].niterations = nits[j]; stats[j].converged = conv[j];
+            stats[j].bnrm2 = bnrm2; stats[j].r0nrm2 = bnrm2; stats[j].rnrm2 = rn[j];
+        }
+    }
+    cg->bnrm2 = cg->r0nrm2 = sqrt((double) nshifts * bb); cg->rnrm2 = sqrt(sr);
+    const double te = wall();
+    OK(download_block_vec(pv, X, pv->d_mx, nshifts, K, errcode));
     pv->last_d2h_ms = 1e3 * (wall() - te);
     CU(cudaGetLastError());
     return status;

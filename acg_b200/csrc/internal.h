@@ -377,6 +377,35 @@ ACGB200_MULTI_LAUNCHER int acgb200_cg_multi_update_xp(int n, int k, struct acgb2
 /* acc[j] += sum_i x[i*k + j]^2 */
 ACGB200_MULTI_LAUNCHER int acgb200_dot_multi(int n, int k, const double *x, double *acc, cudaStream_t stream);
 
+/* ------------------------------------------------------------------------
+ * Shifted systems (acgsolvercuda_solve_shifted): one seed CG on A drives
+ * (A + sigma_j I) x_j = b for K shifts (multi-shift CG).  The seed runs the
+ * single-vector classic loop on d_r, d_p, d_t; X_j and P_j live in block
+ * vectors of width K (d_mx, d_mp), with the same padding and active-column
+ * mask (ctrl.pad0) as the multi-vector loop.  Per-shift scalars are
+ * double-buffered by iteration parity: iteration k reads slot k&1 and block 0
+ * of its update writes slot (k&1)^1, so no kernel reads a slot it writes.
+ * ------------------------------------------------------------------------ */
+struct acgb200_sstate {
+    double zeta[2][ACGB200_MAXK];       /* zeta_k of shift j in slot k&1 (zeta_0 = 1) */
+    double zeta_prev[2][ACGB200_MAXK];  /* zeta_{k-1} in slot k&1 (zeta_{-1} = 1) */
+    double ab_prev[2][2];               /* the seed's {alpha_{k-1}, beta_{k-1}} in slot k&1 ({1, 0} at k = 0) */
+    double sigma[ACGB200_MAXK];         /* the shifts */
+    double tol[ACGB200_MAXK];           /* stop shift j when |zeta_j| ||r|| < tol[j] (0: never) */
+    double final_rnrm2[ACGB200_MAXK];   /* |zeta_j| ||r|| of the shift's last iterate */
+    int nits[ACGB200_MAXK];             /* iterations the shift ran */
+    int conv[ACGB200_MAXK];             /* 1: the shift met its tolerance */
+};
+/* set-up: r = p = b, X_j = 0 and P_j = b for all k columns */
+ACGB200_MULTI_LAUNCHER int acgb200_shift_setup(int n, int k, const double *b, double *r, double *p, double *x, double *pk,
+                                               cudaStream_t stream);
+/* after acgb200_cg_update_r: the seed's p = r + beta p, and for each active shift X_j += alpha_j P_j ;
+ * P_j = zeta_{k+1,j} r + beta_j P_j.  Block 0 advances the control word, applies each shift's
+ * convergence test and clears the next product's (p,Ap) accumulator. */
+ACGB200_MULTI_LAUNCHER int acgb200_cg_shift_update(int n, int k, struct acgb200_devstate *st, struct acgb200_sstate *ss,
+                                                   int cin, int cout, const double *r, double *p, double *x, double *pk,
+                                                   cudaStream_t stream);
+
 /* setup-time helpers */
 int acgb200_dot(int n, const double *x, const double *y, double *acc, cudaStream_t stream); /* acc += x.y */
 int acgb200_dot2(int n, const double *r, const double *w, double *acc2, cudaStream_t stream); /* acc2[0]+=r.r, acc2[1]+=w.r */

@@ -1684,6 +1684,144 @@ dot_multi_kernel(int n, const double *__restrict__ x, double *acc)
     colpair_sum_add<K>(a0, a1, red, acc, (1u << K) - 1u);
 }
 
+/* ---- shifted systems (multi-shift CG) ----------------------------------------------------------- */
+
+struct ShiftScalars { double zn, as, bs; };
+
+/* zeta_{k+1}, alpha^sigma_k = alpha_k zeta_{k+1}/zeta_k and beta^sigma_k = beta_k (zeta_{k+1}/zeta_k)^2 of one
+ * shift, from the seed's alpha_k, beta_k, alpha_{k-1}, beta_{k-1} and the shift's zeta_k, zeta_{k-1}.  Explicit
+ * fma, so that sigma = 0 gives zeta = 1, alpha^sigma = alpha and beta^sigma = beta exactly. */
+__device__ __forceinline__ ShiftScalars shift_scalars(double al, double be, double alp, double bep, double z, double zp,
+                                                      double sg)
+{
+    ShiftScalars o;
+    const double den = fma(al * bep, zp - z, zp * alp * fma(sg, al, 1.0));
+    o.zn = z * zp * alp / den;
+    const double q = o.zn / z;
+    o.as = al * q;
+    o.bs = be * q * q;
+    return o;
+}
+
+/* set-up of solve_shifted: r = p = b ; X_j = 0 ; P_j = b (all K columns) */
+template <int K>
+__global__ void __launch_bounds__(BLAS1_THREADS)
+shift_setup_kernel(int n, const double *__restrict__ b, double *__restrict__ r, double *__restrict__ p,
+                   double *__restrict__ x, double *__restrict__ pk)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const double v = b[i];
+        r[i] = v; p[i] = v;
+#pragma unroll
+        for (int j = 0; j < K; j++) { x[(long long) i * K + j] = 0.0; pk[(long long) i * K + j] = v; }
+    }
+}
+
+/* One iteration's update behind cg_update_r_kernel (which left r = r_{k+1} and (r_{k+1},r_{k+1}) in rr_loc[s^1]):
+ *   seed:            p = r + beta_k p
+ *   active shift j:  X_j += alpha^sigma_k P_j ;  P_j = zeta_{k+1} r + beta^sigma_k P_j
+ * A warp works on 32 row pairs at a time.  Lane l loads the seed's r and p of one pair, once, and updates p;
+ * the X and P entries of the 32 pairs (32 K contiguous double2) are then read by consecutive lanes, each lane
+ * taking the slots l, l + 32, ..., l + 32 (K - 1).  Since K divides 32, a lane always sees the same double2
+ * slot e = l mod K of a pair, i.e. the same two columns (K = 1: one column, two rows), so it derives the
+ * scalars of those two shifts only; the r value of the slot's row comes from the owning lane by shuffle.
+ * Block 0 keeps the books: the next iteration's slot of the per-shift state, each active shift's test
+ * |zeta_{k+1}| ||r_{k+1}|| < tol_j (a shift that meets it leaves the mask, its x the iterate just formed),
+ * the next product's (p,Ap) accumulator, and the control word (done when no shift is left). */
+template <int K>
+__global__ void __launch_bounds__(BLAS1_THREADS)
+cg_shift_update_kernel(int n, acgb200_devstate *st, acgb200_sstate *ss, int cin, int cout,
+                       const double *__restrict__ r, double *__restrict__ p, double *__restrict__ x,
+                       double *__restrict__ pk)
+{
+    pdl_prologue();
+    const Gate g = gate_read(&st->ctrl[cin], st);
+    const int s = g.iter & 1;
+    const unsigned mask = (unsigned) st->ctrl[cin].pad0;
+    const double rr = st->rr_loc[s], rrn = st->rr_loc[s ^ 1], pap = st->pap_loc[s];
+    const double al = rr / pap, be = rrn / rr;
+    const double alp = ss->ab_prev[s][0], bep = ss->ab_prev[s][1];
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        acgb200_ctrl c = st->ctrl[cin];
+        if (g.active) {
+            unsigned next = mask;
+            c.iter = g.iter + 1;
+            const double rn = sqrt(rrn);
+            for (int j = 0; j < K; j++) {
+                if (!(mask >> j & 1u)) continue;
+                const double z = ss->zeta[s][j];
+                const ShiftScalars o = shift_scalars(al, be, alp, bep, z, ss->zeta_prev[s][j], ss->sigma[j]);
+                ss->zeta[s ^ 1][j] = o.zn;
+                ss->zeta_prev[s ^ 1][j] = z;
+                const double nrm = fabs(o.zn) * rn;
+                ss->nits[j] = g.iter + 1;
+                ss->final_rnrm2[j] = nrm;
+                /* acg/cgcuda.c:1008-1012 per shift: ||r_j|| < tol_j, strictly */
+                if (ss->tol[j] > 0.0 && nrm < ss->tol[j]) { next &= ~(1u << j); ss->conv[j] = 1; }
+            }
+            ss->ab_prev[s ^ 1][0] = al;
+            ss->ab_prev[s ^ 1][1] = be;
+            st->pap_loc[s ^ 1] = 0.0;       /* accumulator of the next product */
+            c.pad0 = (int) next;
+            if (next == 0) c.done = 1;
+        }
+        st->ctrl[cout] = c;
+    }
+    if (!g.active) return;
+    const int lane = threadIdx.x & 31;
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
+    const int e = lane & (K - 1);                           /* this lane's double2 slot of a row pair */
+    const int c0 = (2 * e) & (K - 1), c1 = K == 1 ? 0 : c0 + 1;
+    const bool hi = K > 1 && 2 * e >= K;                    /* the slot holds the pair's second row */
+    const bool act0 = mask >> c0 & 1u, act1 = mask >> c1 & 1u;
+    ShiftScalars o0 = { 0.0, 0.0, 0.0 }, o1 = o0;
+    if (act0) o0 = shift_scalars(al, be, alp, bep, ss->zeta[s][c0], ss->zeta_prev[s][c0], ss->sigma[c0]);
+    if (act1) o1 = shift_scalars(al, be, alp, bep, ss->zeta[s][c1], ss->zeta_prev[s][c1], ss->sigma[c1]);
+    const int npairs = n >> 1;
+    const double2 *r2 = reinterpret_cast<const double2 *>(r);
+    double2 *p2 = reinterpret_cast<double2 *>(p);
+    double2 *x2 = reinterpret_cast<double2 *>(x);
+    double2 *q2 = reinterpret_cast<double2 *>(pk);
+    for (int wb = warp * 32; wb < npairs; wb += nwarps * 32) {          /* uniform across the warp */
+        const int i = wb + lane;
+        double2 rv = make_double2(0.0, 0.0);
+        if (i < npairs) {
+            rv = r2[i];
+            double2 pv = p2[i];
+            pv.x = fma(be, pv.x, rv.x);
+            pv.y = fma(be, pv.y, rv.y);
+            p2[i] = pv;
+        }
+#pragma unroll
+        for (int t = 0; t < K; t++) {
+            const int m = lane + 32 * t;                    /* double2 slot among the warp's 32 K */
+            const int pr = m / K;                           /* its row pair, relative to wb */
+            const double rx = __shfl_sync(0xffffffffu, rv.x, pr);
+            const double ry = __shfl_sync(0xffffffffu, rv.y, pr);
+            if (!(act0 || act1) || wb + pr >= npairs) continue;
+            const double ra = hi ? ry : rx, rb = K == 1 ? ry : ra;
+            const long long o = (long long) wb * K + m;
+            double2 xv = x2[o], qv = q2[o];
+            if (act0) { xv.x = fma(o0.as, qv.x, xv.x); qv.x = fma(o0.bs, qv.x, o0.zn * ra); }
+            if (act1) { xv.y = fma(o1.as, qv.y, xv.y); qv.y = fma(o1.bs, qv.y, o1.zn * rb); }
+            x2[o] = xv;
+            q2[o] = qv;
+        }
+    }
+    if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0) {
+        const double rv = r[n - 1];
+        p[n - 1] = fma(be, p[n - 1], rv);
+        for (int j = 0; j < K; j++) {
+            if (!(mask >> j & 1u)) continue;
+            const ShiftScalars oj = shift_scalars(al, be, alp, bep, ss->zeta[s][j], ss->zeta_prev[s][j], ss->sigma[j]);
+            const long long o = (long long) (n - 1) * K + j;
+            const double qv = pk[o];
+            x[o] = fma(oj.as, qv, x[o]);
+            pk[o] = fma(oj.bs, qv, oj.zn * rv);
+        }
+    }
+}
+
 /* ------------------------------------------------------------------------ */
 /* host-side launchers (C linkage)                                           */
 /* ------------------------------------------------------------------------ */
@@ -2115,6 +2253,27 @@ extern "C" int acgb200_dot_multi(int n, int k, const double *x, double *acc, cud
     static int occ[9];
 #define CALL(K) (dot_multi_kernel<K><<<blas1_grid(n * K, (const void *) dot_multi_kernel<K>, &occ[K]), BLAS1_THREADS, 0, stream>>>(n, x, acc), \
                  cudaGetLastError())
+    return (int) MULTI_K_DISPATCH(k, CALL);
+#undef CALL
+}
+
+extern "C" int acgb200_shift_setup(int n, int k, const double *b, double *r, double *p, double *x, double *pk,
+                                   cudaStream_t stream)
+{
+    static int occ[9];
+#define CALL(K) (shift_setup_kernel<K><<<blas1_grid(n, (const void *) shift_setup_kernel<K>, &occ[K]), BLAS1_THREADS, 0, stream>>>( \
+                     n, b, r, p, x, pk), cudaGetLastError())
+    return (int) MULTI_K_DISPATCH(k, CALL);
+#undef CALL
+}
+
+/* grid: as blas1_grid over the n rows (one row pair per thread, 32 pairs per warp) */
+extern "C" int acgb200_cg_shift_update(int n, int k, acgb200_devstate *st, acgb200_sstate *ss, int cin, int cout,
+                                       const double *r, double *p, double *x, double *pk, cudaStream_t stream)
+{
+    static int occ[9];
+#define CALL(K) launch_chain(cg_shift_update_kernel<K>, blas1_grid(n, (const void *) cg_shift_update_kernel<K>, &occ[K]), \
+                             BLAS1_THREADS, 0, stream, n, st, ss, cin, cout, r, p, x, pk)
     return (int) MULTI_K_DISPATCH(k, CALL);
 #undef CALL
 }

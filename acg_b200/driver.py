@@ -45,6 +45,9 @@ def parse_args(argv=None):
     ap.add_argument("--nrhs", type=int, default=None,
                     help="solve K (1-8) seeded right-hand sides at once: classic CG per column, one pass over the matrix per "
                          "iteration for all of them (acgsolvercuda_solve_multi; one process only)")
+    ap.add_argument("--shifts", default=None, metavar="S0,S1,...",
+                    help="solve (A + s_j I) x_j = b for 1-8 comma-separated shifts s_j >= 0 at once from x0 = 0: one CG "
+                         "on A drives every shifted system (acgsolvercuda_solve_shifted; one process, classic solver)")
     ap.add_argument("--seed", type=int, default=1)
     ap.add_argument("--output-comm-matrix", metavar="PATH", help="write the halo send-count matrix (cuda/acg-cuda.c:1713-1775)")
     ap.add_argument("--output-solution", metavar="PATH", help="write x as a Matrix Market vector (text)")
@@ -141,6 +144,33 @@ def solve_multi(args, A, cg, n, log):
     return code
 
 
+def solve_shifted(args, A, cg, log):
+    """The --shifts run: one solve_shifted call, the solver report, then per shift its iterations, its
+    recursively updated residual norm and the true residual ||b - (A + s_j I) x_j||."""
+    b, _ = local_rhs(args, A, A.c.nprows)
+    code, X, cols = cg.solve_shifted(b, args.shifts, maxits=args.max_iterations, residualatol=args.residual_atol,
+                                     residualrtol=args.residual_rtol, warmup=args.warmup)
+    log(cg.report())
+    log(f"shifts: {len(args.shifts)}")
+    import scipy.sparse as sp
+    n = A.c.nownedrows
+    rp = A.frowptr[:n + 1]
+    F = sp.csr_matrix((A.fa[:rp[n]], A.fcolidx[:rp[n]] - A.c.rowidxbase, rp), shape=(n, n))
+    for j, (sigma, c) in enumerate(zip(args.shifts, cols)):
+        true = float(np.linalg.norm(b - F @ X[:, j] - sigma * X[:, j]))
+        log(f"  shift {j} ({sigma:.6g}): iterations {c['niterations']} converged {c['converged']} "
+            f"residual 2-norm {c['rnrm2']:.15g} true residual 2-norm {true:.15g} "
+            f"relative {true / c['bnrm2'] if c['bnrm2'] else 0.0:.3e}")
+    if args.output_solution:
+        from . import mtxio
+        for j in range(len(args.shifts)):
+            root, ext = os.path.splitext(args.output_solution)
+            mtxio.write_vector(f"{root}.{j}{ext}", X[:, j], binary=False)
+    if code != 0:
+        log(f"acg_b200.driver: solver returned {code} (not converged)")
+    return code
+
+
 def main(argv=None):
     args = parse_args(argv)
     # torchrun exports OMP_NUM_THREADS=1 unless the caller set it; the ingest and the full-storage
@@ -160,6 +190,23 @@ def main(argv=None):
             raise SystemExit("--nrhs runs in one process (one GPU, the whole matrix)")
         if args.solver != "acg":
             raise SystemExit("--nrhs solves with classic CG (--solver acg)")
+    if args.shifts is not None:
+        try:
+            args.shifts = [float(v) for v in args.shifts.split(",")]
+        except ValueError:
+            raise SystemExit(f"--shifts: not a comma-separated list of numbers: {args.shifts!r}")
+        if not 1 <= len(args.shifts) <= 8:
+            raise SystemExit("--shifts takes between 1 and 8 shifts")
+        if not all(np.isfinite(v) and v >= 0 for v in args.shifts):
+            raise SystemExit("--shifts must be finite and >= 0")
+        if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            raise SystemExit("--shifts runs in one process (one GPU, the whole matrix)")
+        if args.solver != "acg":
+            raise SystemExit("--shifts solves with classic CG (--solver acg)")
+        if args.nrhs is not None:
+            raise SystemExit("--shifts and --nrhs cannot be combined (one right-hand side for all shifts)")
+        if args.manufactured_solution:
+            raise SystemExit("--shifts and --manufactured-solution cannot be combined (b = 1 for every shift)")
     rank, world, _local = abdist.init_process(backend="gloo")
     log = (lambda *a: print(*a, file=sys.stderr, flush=True)) if rank == 0 else (lambda *a: None)
     if world > 1 and not args.binary:
@@ -199,6 +246,11 @@ def main(argv=None):
         raise SystemExit("acg_b200.driver: no CUDA device (the solver has no CPU path; --dry-run stops before it)")
     comm = abdist.nccl_comm(rank, world)
     cg = SolverCuda(A, comm)
+    if args.shifts is not None:
+        code = solve_shifted(args, A, cg, log)
+        cg.free()
+        comm.destroy()
+        return 0 if code == 0 else 1
     if args.nrhs is not None:
         code = solve_multi(args, A, cg, n, log)
         cg.free()

@@ -77,6 +77,29 @@ ACG_API int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acg
 ACG_API int acgsolvercuda_spmm_mode(struct acgsolvercuda *cg, int mode, int nrhs, const double *X, const double *B,
                                     double *Y, double *dots);
 
+/* A family of shifted systems (A + shifts[j] I) x_j = b, j < nshifts (1..8), in one Krylov space
+ * (multi-shift CG): one classic CG on A -- one single-vector product per iteration for all shifts, no
+ * extra dot products -- drives every shifted system through the zeta recurrence, each shift adding
+ * two vector updates.  A is the operator the solver holds (with the eps it was built with).  b is a
+ * host array of nownedrows doubles; X a host array of nownedrows x nshifts doubles, row-major (entry
+ * (i, j) at i*nshifts + j), OUTPUT ONLY: the initial guess is zero for every shift (the method needs
+ * collinear initial residuals) and X's contents on entry are ignored.  Shift j stops by the rule
+ * acgsolvercuda_solvempi applies to that system alone from x0 = 0: tol = threshold(atol, rtol, ||b||),
+ * strict ||r_j|| < tol with ||r_j|| = |zeta_j| ||r|| the recursively updated residual norm; a shift that
+ * meets it is frozen at that iterate (0 iterations if ||b|| meets it).  The loop ends when every shift
+ * has stopped or at maxits; the seed need not converge itself.  Shifts must be finite and >= 0 (every
+ * shifted system then at least as well conditioned as A): anything else, or nshifts outside [1, 8],
+ * gives ACG_ERR_INVALID_VALUE.  One GPU, unpartitioned matrix: ghost rows or a communicator of more than
+ * one rank give ACG_ERR_NOT_SUPPORTED.  Returns ACG_ERR_NOT_CONVERGED if a shift did not converge under a
+ * non-zero tolerance.  In *cg: niterations is the iterations the loop ran, bnrm2 / r0nrm2 / rnrm2 the
+ * Frobenius norms over the shifts; stats (may be NULL, nshifts entries) gets each shift's iterations,
+ * converged flag, ||b||, r0 = ||b|| and final |zeta_j| ||r||.  `warmup` iterations run first on scratch
+ * state; the results do not depend on them. */
+ACG_API int acgsolvercuda_solve_shifted(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A,
+                                        int nshifts, const double *shifts, const double *b, double *X,
+                                        int maxits, double residualatol, double residualrtol, int warmup,
+                                        struct acgb200_colstats *stats);
+
 struct acgb200_info {
     int spmv_lanes_per_row, spmv_rows_cap, spmv_nnz_cap, spmv_stages;
     int spmv_ntiles, spmv_nlong, spmv_grid, spmv_smem_bytes;
