@@ -6,4 +6,4 @@ This package is only the ctypes mirror of that interface plus host-side
 synthetic matrix generators.
 """
 from . import matgen  # noqa: F401
-from .api import (AcgError, Comm, SolverCuda, SymCsrMatrix, Vector, build, lib, mtx_info, set_option, spmv_plan_host, patterns_host, slices_host, merge_plan_host)  # noqa: F401
+from .api import (AcgError, Comm, SolverCuda, SymCsrMatrix, Vector, build, lib, mtx_info, set_option, spmv_plan_host, patterns_host, slices_host, symdiag_host, merge_plan_host)  # noqa: F401

@@ -127,7 +127,8 @@ class acgb200_info(C.Structure):
                                                                                   ("spmv_slice_exc", C.c_int)] + \
         [(n, C.c_int) for n in ("spmv_threads", "spmv_unroll", "spmv_slice_threads", "spmv_merge_threads",
                                 "spmv_merge_grid", "spmv_merge_stages")] + \
-        [("spmv_slice_value_bytes", C.c_int64), ("spmv_slice_nnz", C.c_int64)]
+        [("spmv_slice_value_bytes", C.c_int64), ("spmv_slice_nnz", C.c_int64)] + \
+        [("spmv_symdiag_diagonals", C.c_int), ("spmv_symdiag_bytes", C.c_int64)]
 
 
 class acgb200_colstats(C.Structure):
@@ -161,7 +162,7 @@ EXPORTS = [
     "acgsolvercuda_fwrite",
     "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_solve_multi", "acgsolvercuda_spmm_mode", "acgsolvercuda_solve_shifted", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
     "acgb200_nccl_unique_id", "acgb200_comm_init_rank", "acgb200_comm_destroy",
-    "acgb200_host_register", "acgb200_host_unregister", "acgb200_spmv_plan_host", "acgb200_spmv_plan_host2", "acgb200_slices_host", "acgb200_merge_plan_host", "acgb200_p2p_inverse_map", "acgb200_patterns_host", "acgb200_stencil_part",
+    "acgb200_host_register", "acgb200_host_unregister", "acgb200_spmv_plan_host", "acgb200_spmv_plan_host2", "acgb200_slices_host", "acgb200_symdiag_host", "acgb200_merge_plan_host", "acgb200_p2p_inverse_map", "acgb200_patterns_host", "acgb200_stencil_part",
     "acgb200_mtx_info", "acgb200_mtx_read", "acgb200_mtx_read_part", "acgb200_comm_matrix_row", "acgb200_partition_rows_grid", "acgb200_grid_factors", "acgb200_rmat_spd",
 ]
 
@@ -255,6 +256,7 @@ def lib() -> C.CDLL:
     L.acgb200_merge_plan_host.argtypes = [C.c_int, i64p, C.c_int, i32p, C.c_int, i32p, P(C.c_int), P(C.c_int)]
     L.acgb200_slices_host.argtypes = [C.c_int, C.c_int, i64p, C.c_void_p, i32p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p]
+    L.acgb200_symdiag_host.argtypes = [C.c_int, C.c_int, i64p, i32p, i32p, i32p, i32p, i32p]
     L.acgb200_spmv_plan_host.argtypes = [C.c_int, i64p, P(acgb200_info), i32p, C.c_int, i32p, C.c_int]
     L.acgb200_comm_init_rank.argtypes = [P(acgcomm), C.c_int, C.c_void_p, C.c_int, P(C.c_int)]
     L.acgb200_comm_destroy.argtypes = [P(acgcomm)]
@@ -329,6 +331,29 @@ def slices_host(rowptr, colidx, cover_hi=None) -> dict:
     return dict(nslices=ns, slices=slices4[:4 * ns].reshape(ns, 4).copy(), covered=covered[:nsl].astype(bool),
                 blocks=int(totals[1]), nnz=int(totals[2]), rows=int(totals[3]), lpad=int(totals[4]), npat=int(totals[5]),
                 spatoff=spatoff, patid=patid[:n], nexc=int(exc2[0]), excnnz=int(exc2[1]))
+
+
+SYMDIAG_REASONS = ("eligible", "no slices", "exception rows", "unsorted row", "too many offsets", "no gain", "too large")
+
+
+def symdiag_host(rowptr, colidx, cover_hi=None) -> dict:
+    """The mirrored-diagonal plan acgsolvercuda_init would use for the pattern slices (slices.c), computed on
+    the host: ``reason`` (one of SYMDIAG_REASONS; "eligible" means the layout is used if the values pass the
+    device's symmetry check), the offsets ``O`` of the covered rows, the stored diagonals ``D``, and for an
+    eligible plan the ``margin``, ``stride`` and per-entry ``voff`` / ``coff`` of the kernel's addressing."""
+    rowptr = np.ascontiguousarray(rowptr, dtype=np.int64)
+    colidx = np.ascontiguousarray(colidx, dtype=np.int32)
+    n = len(rowptr) - 1
+    info = np.zeros(5, np.int32)
+    o = np.zeros(64, np.int32)
+    d = np.zeros(64, np.int32)
+    tab = np.zeros(128, np.int32)
+    _check(lib().acgb200_symdiag_host(n, n if cover_hi is None else cover_hi, rowptr, colidx, info, o, d, tab),
+           "acgb200_symdiag_host")
+    no, nd = int(info[1]), int(info[2])
+    t = tab[:2 * no].reshape(no, 2)
+    return dict(reason=SYMDIAG_REASONS[int(info[0])], O=o[:no].copy(), D=d[:nd].copy(), margin=int(info[3]),
+                stride=int(info[4]), voff=t[:, 0].copy(), coff=t[:, 1].copy())
 
 
 def spmv_plan_host(rowptr, colidx=None) -> dict:

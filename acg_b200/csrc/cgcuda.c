@@ -60,8 +60,11 @@ static struct {
     int merge_items, merge_threads, merge_max_ctas, merge_stages;   /* their shape (0 = default) */
     int spmv_slices;    /* 1: pattern slices (slices.c) -- index-free slice-major storage of the rows that repeat a pattern */
     int slice_ub, slice_threads, slice_max_ctas;   /* slice kernel shape overrides (0 = default) */
+    int spmv_symdiag;   /* 1: mirrored diagonals for the slice-covered rows when the matrix allows (slices.c), 0: off */
+    int symdiag_evict_first;   /* 1: L2 evict-first policy on the stored diagonals (A/B; the default reuses them in L2) */
     int loaded;
-} cfg = { .check_every = 8, .graph = 1, .redstream = 1, .p2p = 1, .p2p_fuse = 1, .spmv_slices = 1, .spmv_merge = -1 };
+} cfg = { .check_every = 8, .graph = 1, .redstream = 1, .p2p = 1, .p2p_fuse = 1, .spmv_slices = 1, .spmv_merge = -1,
+          .spmv_symdiag = 1 };
 
 static void cfg_load(void)
 {
@@ -94,6 +97,8 @@ static void cfg_load(void)
     if ((s = getenv("ACGB200_SLICE_UB"))) cfg.slice_ub = atoi(s);
     if ((s = getenv("ACGB200_SLICE_THREADS"))) cfg.slice_threads = atoi(s);
     if ((s = getenv("ACGB200_SLICE_MAX_CTAS"))) cfg.slice_max_ctas = atoi(s);
+    if ((s = getenv("ACGB200_SPMV_SYMDIAG"))) cfg.spmv_symdiag = atoi(s);
+    if ((s = getenv("ACGB200_SYMDIAG_EVICT_FIRST"))) cfg.symdiag_evict_first = atoi(s);
     acgb200_blas1_set_ctas_per_sm(cfg.blas1_ctas);
     acgb200_set_pdl(cfg.pdl);
 }
@@ -126,6 +131,8 @@ int acgb200_set_option(const char *key, int value)
     else if (!strcmp(key, "slice_ub")) cfg.slice_ub = value;
     else if (!strcmp(key, "slice_threads")) cfg.slice_threads = value;
     else if (!strcmp(key, "slice_max_ctas")) cfg.slice_max_ctas = value;
+    else if (!strcmp(key, "spmv_symdiag")) cfg.spmv_symdiag = value;
+    else if (!strcmp(key, "symdiag_evict_first")) cfg.symdiag_evict_first = value;
     else return ACG_ERR_INVALID_VALUE;
     return ACG_SUCCESS;
 }
@@ -265,6 +272,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
         for (int i = 0; i < 4; i++) if (pv->graph[i]) cudaGraphExecDestroy(pv->graph[i]);
         cudaFree(pv->plan.d_tiles); cudaFree(pv->plan.d_longrows); cudaFree(pv->plan.d_long_scratch); cudaFree(pv->plan.d_medrows);
         cudaFree(pv->plan.d_slices); cudaFree(pv->plan.d_sval); cudaFree(pv->plan.d_spatoff); cudaFree(pv->plan.d_spatid);
+        cudaFree(pv->plan.d_hval); cudaFree(pv->plan.d_symdiag_bad);
         cudaFree(pv->plan.d_mtiles); cudaFree(pv->plan.d_msplit); cudaFree(pv->plan.d_mpart);
         cudaFree(pv->d_st);
         cudaFreeHost(pv->h_ctrl); cudaFreeHost(pv->h_st);
@@ -443,6 +451,32 @@ int acgb200_slices_host(int nrows, int cover_hi, const int64_t *rowptr, const in
         if (sp.nslices > 0) memcpy(spatoff, sp.spatoff, (size_t) sp.npat * (size_t) sp.lpad * sizeof(int));
         if (patid && sp.nslices > 0) memcpy(patid, sp.patid, (size_t) nrows * sizeof(*patid));
         if (exc2) { exc2[0] = sp.nexc; exc2[1] = sp.excnnz; }
+    }
+    acgb200_sliceplan_free(&sp);
+    acgb200_patterns_free(&pat);
+    return err;
+}
+
+/* ext.h: the mirrored-diagonal plan of a CSR matrix's pattern slices, host only (slices.c) */
+int acgb200_symdiag_host(int nrows, int cover_hi, const int64_t *rowptr, const int *colidx, int *info5, int *o, int *d,
+                         int *tab2)
+{
+    struct acgb200_patterns pat;
+    struct acgb200_sliceplan sp;
+    struct acgb200_symdiag sd;
+    int err = acgb200_patterns_build(nrows, rowptr, colidx, 4096, &pat);
+    if (err) return err;
+    err = acgb200_slices_plan(nrows, cover_hi, rowptr, &pat, &sp);
+    if (!err) err = acgb200_symdiag_plan(nrows, &sp, &pat, &sd);
+    if (!err) {
+        int margin = 0, stride = 0;
+        struct acgb200_symdiag_entry tab[ACGB200_SYMDIAG_MAX];
+        if (sd.reason == SYMDIAG_OK) acgb200_symdiag_layout(nrows, &sd, &margin, &stride, tab);
+        info5[0] = sd.reason; info5[1] = sd.no; info5[2] = sd.nd; info5[3] = margin; info5[4] = stride;
+        memcpy(o, sd.o, (size_t) sd.no * sizeof(int));
+        memcpy(d, sd.d, (size_t) sd.nd * sizeof(int));
+        if (sd.reason == SYMDIAG_OK)
+            for (int e = 0; e < sd.no; e++) { tab2[2 * e] = tab[e].voff; tab2[2 * e + 1] = tab[e].coff; }
     }
     acgb200_sliceplan_free(&sp);
     acgb200_patterns_free(&pat);
@@ -712,6 +746,7 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
     if (cfg.spmv_threads > 0) pv->plan.threads = cfg.spmv_threads;
     if (cfg.spmv_unroll > 0) pv->plan.unroll = cfg.spmv_unroll;
     pv->plan.med_thr = cfg.spmv_medium;
+    int slice_domlen = 0;
     {
         struct acgb200_patterns pat;
         struct acgb200_sliceplan sp;
@@ -746,10 +781,27 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
         }
         acgb200_mergeplan_free(&mp);
         if (!err && pv->plan.nslices > 0) {
-            const int d = sp.domlen;
-            pv->plan.slice_ub = cfg.slice_ub > 0 ? cfg.slice_ub : (d % 9 == 0 ? 9 : d % 7 == 0 ? 7 : d % 8 == 0 ? 8 : d % 5 == 0 ? 5 : 8);
+            slice_domlen = sp.domlen;
             pv->plan.slice_threads = cfg.slice_threads > 0 ? cfg.slice_threads : 128;
             pv->plan.slice_max_ctas = cfg.slice_max_ctas;
+        }
+        if (!err && pv->plan.nslices > 0 && cfg.spmv_symdiag) {
+            /* mirrored diagonals: planned here, stored and checked by acgb200_slices_fill below */
+            struct acgb200_symdiag sd;
+            err = acgb200_symdiag_plan(A->nownedrows, &sp, &pat, &sd);
+            if (!err && sd.reason == SYMDIAG_OK) {
+                struct acgb200_spmvplan *pl = &pv->plan;
+                acgb200_symdiag_layout(A->nownedrows, &sd, &pl->symdiag_margin, &pl->symdiag_stride, pl->symdiag_tab);
+                memcpy(pl->symdiag_d, sd.d, (size_t) sd.nd * sizeof(int));
+                pl->symdiag_nd = sd.nd; pl->symdiag_no = sd.no;
+                pl->symdiag_evict_first = cfg.symdiag_evict_first;
+                pl->symdiag_colidx = cg->d_colidx;
+                cudaError_t e = cudaMalloc((void **) &pl->d_hval, (size_t) sd.nd * (size_t) pl->symdiag_stride * sizeof(double));
+                if (!e) e = cudaMalloc((void **) &pl->d_symdiag_bad, sizeof(int));
+                /* "failed" until the device check has run and passed */
+                if (!e) { const int one = 1; e = cudaMemcpy(pl->d_symdiag_bad, &one, sizeof(int), cudaMemcpyHostToDevice); }
+                if (e) { *errcode = (int) e; err = ACG_ERR_CUDA; }
+            }
         }
         acgb200_sliceplan_free(&sp);
         acgb200_patterns_free(&pat);
@@ -757,12 +809,29 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
         if (err) return err;
     }
     pv->plan.max_ctas_per_sm = cfg.spmv_max_ctas;
-    KL(acgb200_spmv_configure(&pv->plan));
     if (pv->plan.nslices > 0) {
-        /* slice-major copy of the covered rows' values, made on the device from the CSR values */
-        KL(acgb200_slices_fill(&pv->plan, cg->d_rowptr, cg->d_a, pv->stream));
+        /* slice-major copy of the covered rows' values, made on the device from the CSR values; with mirrored
+         * diagonals also those and the check that every lower entry equals its mirror bit for bit */
+        struct acgb200_spmvplan *pl = &pv->plan;
+        KL(acgb200_slices_fill(pl, cg->d_rowptr, cg->d_a, pv->stream));
         CU(cudaStreamSynchronize(pv->stream));
+        pl->symdiag_colidx = NULL;
+        if (pl->d_symdiag_bad) {
+            int bad = 1;
+            CU(cudaMemcpy(&bad, pl->d_symdiag_bad, sizeof(int), cudaMemcpyDeviceToHost));
+            CU(cudaFree(pl->d_symdiag_bad));
+            pl->d_symdiag_bad = NULL;
+            if (bad) {
+                /* not exactly symmetric (or the check did not run): the slice kernel reads both triangles */
+                CU(cudaFree(pl->d_hval));
+                pl->d_hval = NULL; pl->symdiag_nd = 0; pl->symdiag_no = 0;
+            }
+        }
+        /* batches that divide the row: |O| for the mirrored diagonals, else the most frequent row length */
+        const int d = pl->symdiag_nd > 0 ? pl->symdiag_no : slice_domlen;
+        pl->slice_ub = cfg.slice_ub > 0 ? cfg.slice_ub : (d % 9 == 0 ? 9 : d % 7 == 0 ? 7 : d % 8 == 0 ? 8 : d % 5 == 0 ? 5 : 8);
     }
+    KL(acgb200_spmv_configure(&pv->plan));
     return ACG_SUCCESS;
 }
 
@@ -2319,5 +2388,7 @@ int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info
     info->spmv_min_bytes = acgb200_spmv_min_bytes(&pv->plan);
     info->spmv_slice_value_bytes = pv->plan.nslices > 0 ? pv->plan.sval_blocks * 32 * (int64_t) sizeof(double) : 0;
     info->spmv_slice_nnz = pv->plan.nslices > 0 ? pv->plan.slice_nnz : 0;
+    info->spmv_symdiag_diagonals = pv->plan.symdiag_nd;
+    info->spmv_symdiag_bytes = (int64_t) pv->plan.symdiag_nd * pv->plan.symdiag_stride * (int64_t) sizeof(double);
     return ACG_SUCCESS;
 }

@@ -34,6 +34,9 @@ struct acgb200_tile {        /* 16 bytes, read as one int4 */
     int nnz_al;              /* padded slice length: multiple of 4, covers the tile's nonzeros */
 };
 
+#define ACGB200_SYMDIAG_MAX 64      /* = SLICE_MAXLEN (slices.c): entries per row of the mirrored-diagonal layout */
+struct acgb200_symdiag_entry { int voff, coff; };   /* value offset (relative to the row), column offset */
+
 struct acgb200_spmvplan {
     int nrows;                       /* rows covered (owned rows) */
     int64_t nnz;
@@ -73,6 +76,19 @@ struct acgb200_spmvplan {
     unsigned short *d_spatid;        /* [nrows] pattern id per row (valid for covered rows) */
     int slice_ub, slice_threads, slice_grid, slice_smem, slice_max_ctas;
     int64_t slice_exc, slice_excnnz; /* exception rows inside slices (columns from the CSR index array) and their nonzeros */
+    /* mirrored diagonals (slices.c, acgb200_symdiag_plan): the slice-covered rows of a symmetric matrix read
+     * their values from symdiag_nd stored upper diagonals, every lower entry from its mirror row
+     * (spmv_symdiag_kernel instead of spmv_slices_kernel); 0: off.  Entry e of a covered row i is
+     * d_hval[symdiag_tab[e].voff + i] times x[i + symdiag_tab[e].coff] (column clamped to [0, nrows)) */
+    int symdiag_nd, symdiag_no;
+    int symdiag_stride;              /* doubles per stored diagonal, the zero front margin included */
+    struct acgb200_symdiag_entry symdiag_tab[ACGB200_SYMDIAG_MAX];
+    int symdiag_d[ACGB200_SYMDIAG_MAX];   /* the stored diagonals D, ascending */
+    int symdiag_margin;              /* zero entries in front of each diagonal (>= max D) */
+    int symdiag_evict_first;         /* 1: stream the stored values with an L2 evict-first policy */
+    double *d_hval;                  /* [symdiag_nd * symdiag_stride] */
+    const int *symdiag_colidx;       /* device CSR columns the fill reads (borrowed, valid during init only) */
+    int *d_symdiag_bad;              /* fill-time symmetry check: 0 passed (written by acgb200_slices_fill) */
     /* merge-path tiles (mergeplan.c): rows [0, merge_rows) of an irregular (power-law) matrix, cut into tiles
      * of merge_items merged items (row ends + nonzeros) and multiplied by spmv_merge_kernel; rows cut by tile
      * boundaries are finished by spmv_merge_fix_kernel from the tiles' partial sums */
@@ -118,7 +134,28 @@ struct acgb200_sliceplan {
 int acgb200_slices_plan(int nrows, int cover_hi, const int64_t *rowptr, const struct acgb200_patterns *pat,
                         struct acgb200_sliceplan *out);
 void acgb200_sliceplan_free(struct acgb200_sliceplan *sp);
-/* fill d_sval from the device CSR values (kernels.cu) */
+
+/* Mirrored diagonals of a slice plan (host, no CUDA).  O: the sorted union of the offsets col - row of the
+ * covered rows; D = {|o| : o in O}, the diagonals stored.  Eligible (reason 0) if the plan has slices and no
+ * exception rows, every covered row's offsets are strictly ascending, |O| <= ACGB200_SYMDIAG_MAX and 8|D|
+ * bytes per covered row are fewer than the slice-major values they replace.  The values themselves are
+ * checked on the device (acgb200_slices_fill). */
+enum { SYMDIAG_OK = 0, SYMDIAG_NO_SLICES, SYMDIAG_EXCEPTIONS, SYMDIAG_UNSORTED, SYMDIAG_TOO_MANY, SYMDIAG_NO_GAIN,
+       SYMDIAG_TOO_LARGE };
+struct acgb200_symdiag {
+    int reason;                      /* SYMDIAG_OK: eligible */
+    int no, nd;
+    int o[ACGB200_SYMDIAG_MAX];      /* O, ascending */
+    int d[ACGB200_SYMDIAG_MAX];      /* D, ascending */
+};
+int acgb200_symdiag_plan(int nrows, const struct acgb200_sliceplan *sp, const struct acgb200_patterns *pat,
+                         struct acgb200_symdiag *out);
+/* the layout of an eligible plan: zero margin and stride of the diagonals, (value, column) offset per entry */
+void acgb200_symdiag_layout(int nrows, const struct acgb200_symdiag *sd, int *margin, int *stride,
+                            struct acgb200_symdiag_entry *tab);
+
+/* fill d_sval from the device CSR values (kernels.cu); with pl->d_hval also the mirrored diagonals and
+ * their symmetry check (pl->d_symdiag_bad) */
 int acgb200_slices_fill(const struct acgb200_spmvplan *pl, const int *d_rowptr, const double *d_a, cudaStream_t stream);
 
 /* row-pattern dictionary (compress.c): rows whose pattern id is not

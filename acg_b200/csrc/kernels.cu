@@ -85,6 +85,13 @@ __device__ __forceinline__ uint64_t l2_policy_evict_first()
     return pol;
 }
 
+__device__ __forceinline__ uint64_t l2_policy_evict_normal()
+{
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+
 /* global -> shared bulk copy; bytes and both addresses are multiples of 16.
  * The matrix streams are read exactly once per SpMV: evict-first keeps them
  * from displacing the x vector in L2. */
@@ -697,6 +704,154 @@ slices_fill_kernel(int nslices, const acgb200_slice *slices, const int *__restri
         const int kb = rowptr[row], len = rowptr[row + 1] - kb;
         double *v = sval + ((size_t) sl.vblk << 5) + lane;
         for (int e = 0; e < sl.len; e++) v[(size_t) e * 32] = e < len ? a[kb + e] : 0.0;
+    }
+}
+
+/* ------------------------------------------------------------------------ */
+/* SpMV over mirrored diagonals (slices.c): each symmetric value read once     */
+/* ------------------------------------------------------------------------ */
+
+struct SymdiagParams {
+    const acgb200_slice *slices;
+    int nslices;
+    int no;                        /* entries per row, |O| */
+    int nrows;                     /* columns are clamped to [0, nrows) */
+    int evict_first;
+    const double *hval;            /* the stored diagonals */
+    acgb200_symdiag_entry tab[ACGB200_SYMDIAG_MAX];   /* (value offset, column offset) per entry, O ascending */
+    const double *x;
+    double *y;
+    const double *b;
+    double *acc;
+    int dotrows;
+    int mode;
+    const acgb200_ctrl *ctrl_in;
+    acgb200_ctrl *ctrl_out;
+    acgb200_devstate *st;
+    int housekeeping;
+};
+
+/*
+ * The slice kernel without per-row patterns: one warp per covered slice, one row per lane, UB value loads
+ * and UB gathers per batch.  Entry e of every row is value hval[voff_e + row] times x[row + coff_e]:
+ * (voff_e, coff_e) is the same for the whole warp, one shared-memory broadcast.  An upper entry (coff >= 0)
+ * is the row's own element of diagonal coff, a lower one the element of diagonal -coff at the mirror row
+ * row + coff -- a copy of the same value, so half of the values are read a second time, from L2: the
+ * grid-stride front spans far more rows than the largest mirror distance (DESIGN section 3a).
+ *
+ * The sum is the row's CSR-order FMA chain of spmv_slices_kernel: entries in ascending offset, one
+ * accumulator; an offset the row does not have contributes fma(0, x[col], sum) == sum.  One difference
+ * follows: such a slot gathers x at its (clamped) column where the slice kernel's padding gathers x[row],
+ * so a non-finite x there makes the row NaN (0 * Inf) where the slice kernel may not.
+ */
+template <int UB, int T>
+__global__ void __launch_bounds__(T)
+spmv_symdiag_kernel(const SymdiagParams P)
+{
+    __shared__ int2 tab_s[ACGB200_SYMDIAG_MAX];
+    __shared__ double red[T / 32];
+    const int tid = threadIdx.x;
+    pdl_prologue();
+    const Gate gate = gate_read(P.ctrl_in, P.st);
+    if (P.ctrl_out && blockIdx.x == 0 && tid == 0 && P.ctrl_in) {
+        *P.ctrl_out = *P.ctrl_in;
+        if (gate.active) {
+            const int s = gate.iter & 1;
+            if (P.housekeeping == 1) P.st->rr_loc[s ^ 1] = 0.0;
+            if (P.housekeeping == 2) { P.st->gd_loc[s ^ 1][0] = 0.0; P.st->gd_loc[s ^ 1][1] = 0.0; }
+        }
+    }
+    if (!gate.active) return;
+    if (tid < P.no) tab_s[tid] = make_int2(P.tab[tid].voff, P.tab[tid].coff);
+    __syncthreads();
+
+    /* L2 policy of the values: see the measurements in DESIGN section 3a */
+    const uint64_t pol = P.evict_first ? l2_policy_evict_first() : l2_policy_evict_normal();
+    const int lane = tid & 31;
+    const int warp = (blockIdx.x * T + tid) >> 5;
+    const int nwarps = (gridDim.x * T) >> 5;
+    const int cmax = P.nrows - 1;
+    const int L = P.no;
+    double dot = 0.0;
+    for (int s = warp; s < P.nslices; s += nwarps) {
+        const int row = __ldg(&P.slices[s].row0) + lane;
+        const double *hv = P.hval + row;
+        double sum = 0.0;
+        int e = 0;
+        for (; e + UB <= L; e += UB) {
+            double vv[UB], xv[UB];
+#pragma unroll
+            for (int u = 0; u < UB; u++) vv[u] = ld_stream(hv + tab_s[e + u].x, pol);
+#pragma unroll
+            for (int u = 0; u < UB; u++) xv[u] = ld_x(P.x + min(max(row + tab_s[e + u].y, 0), cmax));
+            sum = slice_fma<UB>(vv, xv, sum);
+        }
+        if (e < L) {
+            /* last, partial batch: slots past L are neither loaded nor added */
+            double vv[UB], xv[UB];
+#pragma unroll
+            for (int u = 0; u < UB; u++) vv[u] = e + u < L ? ld_stream(hv + tab_s[e + u].x, pol) : 0.0;
+#pragma unroll
+            for (int u = 0; u < UB; u++) xv[u] = e + u < L ? ld_x(P.x + min(max(row + tab_s[e + u].y, 0), cmax)) : 0.0;
+#pragma unroll
+            for (int u = 0; u < UB; u++) if (e + u < L) sum = fma(vv[u], xv[u], sum);
+        }
+        if (P.mode == SPMV_R_B_AX) {
+            const double r = P.b[row] - sum;
+            P.y[row] = r;
+            if (row < P.dotrows) dot = fma(r, r, dot);
+        } else {
+            P.y[row] = sum;
+            if (P.mode == SPMV_Y_AX_DOT && row < P.dotrows) dot = fma(__ldg(P.x + row), sum, dot);
+        }
+    }
+    if (P.acc) {
+        const double v = block_sum(dot, red);
+        if (tid == 0 && v != 0.0) atomicAdd(P.acc, v);
+    }
+}
+
+struct SymdiagList { int d[ACGB200_SYMDIAG_MAX]; };
+
+/* the stored diagonals out of the device CSR arrays (once, at init): element j of diagonal d[k] is
+ * a[j, j + d[k]] for every owned row j; the array was zeroed, margins included */
+__global__ void __launch_bounds__(256)
+symdiag_fill_kernel(int nrows, const int *__restrict__ rowptr, const int *__restrict__ colidx,
+                    const double *__restrict__ a, double *__restrict__ hval, int nd, const SymdiagList D,
+                    int stride, int margin)
+{
+    __shared__ int d_s[ACGB200_SYMDIAG_MAX];
+    if (threadIdx.x < nd) d_s[threadIdx.x] = D.d[threadIdx.x];
+    __syncthreads();
+    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < nrows; j += gridDim.x * blockDim.x) {
+        for (int k = rowptr[j]; k < rowptr[j + 1]; k++) {
+            const int d = colidx[k] - j;
+            if (d < 0) continue;
+            for (int q = 0; q < nd; q++)
+                if (d_s[q] == d) { hval[(size_t) q * stride + margin + j] = a[k]; break; }
+        }
+    }
+}
+
+/* Every covered row's lower entries must be the mirror values the kernel reads, bit for bit: for each
+ * o < 0 in O, a[i, i+o] (or +0.0 where row i has no such entry) against the stored value at the mirror
+ * row.  The rows are sorted (slices.c), so one pass over the row's entries.  Any difference sets *bad. */
+__global__ void __launch_bounds__(256)
+symdiag_check_kernel(SymdiagParams P, const int *__restrict__ rowptr, const int *__restrict__ colidx,
+                     const double *__restrict__ a, int *bad)
+{
+    const long long nt = (long long) P.nslices * 32;
+    for (long long t = blockIdx.x * (long long) blockDim.x + threadIdx.x; t < nt; t += (long long) gridDim.x * blockDim.x) {
+        const int i = P.slices[t >> 5].row0 + (int) (t & 31);
+        int k = rowptr[i];
+        const int ke = rowptr[i + 1];
+        for (int e = 0; e < P.no && P.tab[e].coff < 0; e++) {
+            const int o = P.tab[e].coff;
+            while (k < ke && colidx[k] - i < o) k++;
+            const double want = (k < ke && colidx[k] - i == o) ? a[k] : 0.0;
+            const double got = P.hval[(long long) P.tab[e].voff + i];
+            if (__double_as_longlong(want) != __double_as_longlong(got)) *bad = 1;
+        }
     }
 }
 
@@ -1925,6 +2080,17 @@ static slice_fn slice_variant(int UB, int T, int EXC)
     return NULL;
 }
 
+typedef void (*symdiag_fn)(const SymdiagParams);
+
+/* the mirrored-diagonal kernel for exactly the (UB, T) pairs of slice_variant */
+static symdiag_fn symdiag_variant(int UB, int T)
+{
+#define X(u, t) if (UB == u && T == t) return spmv_symdiag_kernel<u, t>;
+    X(5, 128) X(7, 128) X(8, 128) X(9, 128) X(7, 256) X(8, 256) X(9, 256)
+#undef X
+    return NULL;
+}
+
 typedef void (*merge_fn)(const MergeParams);
 
 static merge_fn merge_variant(int T)
@@ -1972,16 +2138,33 @@ extern "C" int acgb200_spmv_configure(acgb200_spmvplan *pl)
         pl->merge_grid = (int) (mgrid < 1 ? 1 : mgrid);
     }
     if (pl->nslices > 0) {
-        slice_fn sfn = slice_variant(pl->slice_ub, pl->slice_threads, pl->slice_exc > 0);
+        /* the mirrored-diagonal kernel, when the plan has them, takes the slice kernel's place and grid rule */
+        const void *sfn = pl->symdiag_nd > 0 ? (const void *) symdiag_variant(pl->slice_ub, pl->slice_threads)
+                                             : (const void *) slice_variant(pl->slice_ub, pl->slice_threads, pl->slice_exc > 0);
         if (!sfn) return (int) cudaErrorInvalidConfiguration;
-        pl->slice_smem = ((pl->slice_npat * pl->slice_lpad + 3) & ~3) * (int) sizeof(int);
-        err = cudaFuncSetAttribute((const void *) sfn, cudaFuncAttributeMaxDynamicSharedMemorySize, pl->slice_smem);
+        pl->slice_smem = pl->symdiag_nd > 0 ? 0 : ((pl->slice_npat * pl->slice_lpad + 3) & ~3) * (int) sizeof(int);
+        err = cudaFuncSetAttribute(sfn, cudaFuncAttributeMaxDynamicSharedMemorySize, pl->slice_smem);
         if (err) return (int) err;
         int sper = 0;
-        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&sper, (const void *) sfn, pl->slice_threads, pl->slice_smem);
+        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&sper, sfn, pl->slice_threads, pl->slice_smem);
         if (err) return (int) err;
         if (sper < 1) sper = 1;
         if (pl->slice_max_ctas > 0 && sper > pl->slice_max_ctas) sper = pl->slice_max_ctas;
+        if (pl->symdiag_nd > 0 && pl->slice_max_ctas <= 0) {
+            /* The lower entries are read from L2 only if a value is still there when its mirror row reads it.
+             * The grid-stride front -- one slice per resident warp -- spans far more rows than the largest
+             * mirror distance, and its rows' bytes (8 |D| + 16 per row) are what passes through L2 between the
+             * two reads: keep them within half of the L2.  C3 (14 diagonals): 12 of the 16 CTAs of 128
+             * threads the registers allow, 1026-1029 it/s against 937-939 with 16 (H100 SXM, 400 W, DESIGN
+             * section 3a); C2 (4 diagonals) stays at 16. */
+            int dev = 0, l2 = 0;
+            if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev) == cudaSuccess && l2 > 0) {
+                const long long row_bytes = 8LL * pl->symdiag_nd + 16;
+                long long cap = (long long) l2 / 2 / ((long long) acgb200_num_sms() * pl->slice_threads * row_bytes);
+                if (cap < 1) cap = 1;
+                if (sper > cap) sper = (int) cap;
+            }
+        }
         long long sgrid = (long long) acgb200_num_sms() * sper;
         const long long need = ((long long) pl->nslices * 32 + pl->slice_threads - 1) / pl->slice_threads;
         if (sgrid > need) sgrid = need;
@@ -1997,6 +2180,23 @@ extern "C" int acgb200_slices_fill(const acgb200_spmvplan *pl, const int *d_rowp
     const long long cap = (long long) acgb200_num_sms() * 8;
     if (grid > cap) grid = cap;
     slices_fill_kernel<<<(int) grid, 256, 0, stream>>>(pl->nslices, pl->d_slices, d_rowptr, d_a, pl->d_sval);
+    cudaError_t err = cudaGetLastError();
+    if (err || pl->symdiag_nd <= 0 || !pl->d_hval || !pl->symdiag_colidx || !pl->d_symdiag_bad) return (int) err;
+    /* mirrored diagonals: zero (margins and absent entries), fill from every owned row, then check */
+    err = cudaMemsetAsync(pl->d_hval, 0, (size_t) pl->symdiag_nd * (size_t) pl->symdiag_stride * sizeof(double), stream);
+    if (!err) err = cudaMemsetAsync(pl->d_symdiag_bad, 0, sizeof(int), stream);
+    if (err) return (int) err;
+    SymdiagParams S;
+    memset(&S, 0, sizeof(S));
+    S.slices = pl->d_slices; S.nslices = pl->nslices; S.no = pl->symdiag_no; S.nrows = pl->nrows; S.hval = pl->d_hval;
+    memcpy(S.tab, pl->symdiag_tab, sizeof(S.tab));
+    SymdiagList D;
+    memcpy(D.d, pl->symdiag_d, sizeof(D.d));
+    long long fgrid = ((long long) pl->nrows + 255) / 256;
+    if (fgrid > cap) fgrid = cap;
+    symdiag_fill_kernel<<<(int) (fgrid < 1 ? 1 : fgrid), 256, 0, stream>>>(pl->nrows, d_rowptr, pl->symdiag_colidx, d_a, pl->d_hval,
+                                                                          pl->symdiag_nd, D, pl->symdiag_stride, pl->symdiag_margin);
+    symdiag_check_kernel<<<(int) grid, 256, 0, stream>>>(S, d_rowptr, pl->symdiag_colidx, d_a, pl->d_symdiag_bad);
     return (int) cudaGetLastError();
 }
 
@@ -2028,7 +2228,17 @@ extern "C" int acgb200_spmv_launch(const acgb200_spmvargs *a, cudaStream_t strea
             if (fe) return (int) fe;
         }
     }
-    if (pl->nslices > 0) {
+    if (pl->nslices > 0 && pl->symdiag_nd > 0) {
+        SymdiagParams S;
+        S.slices = pl->d_slices; S.nslices = pl->nslices; S.no = pl->symdiag_no; S.nrows = pl->nrows;
+        S.evict_first = pl->symdiag_evict_first; S.hval = pl->d_hval;
+        memcpy(S.tab, pl->symdiag_tab, sizeof(S.tab));
+        S.x = a->x; S.y = a->y; S.b = a->b; S.acc = a->acc; S.dotrows = a->dotrows; S.mode = a->mode;
+        S.ctrl_in = a->ctrl_in; S.ctrl_out = slices_forward ? a->ctrl_out : NULL; S.st = a->st; S.housekeeping = a->housekeeping;
+        const cudaError_t le = launch_chain(symdiag_variant(pl->slice_ub, pl->slice_threads), pl->slice_grid, pl->slice_threads,
+                                            (size_t) 0, stream, S);
+        if (le) return (int) le;
+    } else if (pl->nslices > 0) {
         /* first: the tile kernel's last CTA publishes the fused dot, which these rows add into */
         SliceParams S;
         S.slices = pl->d_slices; S.nslices = pl->nslices; S.sval = pl->d_sval;

@@ -12,6 +12,9 @@ int64_t acgb200_spmv_min_bytes(const struct acgb200_spmvplan *pl)
 {
     /* tiles: values + indices + per row: row pointer, y, x; slices: padded values + per row: pattern id, y, x */
     const int64_t tnnz = pl->nnz - pl->slice_nnz, trows = pl->nrows - pl->slice_rows;
+    /* mirrored diagonals: per covered row one value per stored diagonal (the lower entries come again from L2), y, x */
+    if (pl->symdiag_nd > 0)
+        return tnnz * 12 + trows * 20 + (int64_t) pl->slice_rows * (8 * pl->symdiag_nd + 16);
     return tnnz * 12 + trows * 20 + pl->sval_blocks * 256 + (int64_t) pl->slice_rows * 18
            + pl->slice_excnnz * 4 + pl->slice_exc * 8;
 }

@@ -116,3 +116,75 @@ int acgb200_slices_plan(int nrows, int cover_hi, const int64_t *rowptr, const st
     }
     return ACG_SUCCESS;
 }
+
+/*
+ * Mirrored diagonals.  The matrix is symmetric and its full storage mirrors the packed triangle, so
+ * a[i, i+o] with o < 0 is a bit-for-bit copy of a[i+o, i], the entry at offset -o of row i+o.  Of the
+ * covered rows' offsets O only D = {|o|} need storing: diagonal d holds a[j, j+d] of every owned row j
+ * (0 where row j has no such entry), behind a zero margin of at least max D entries.  A covered row then
+ * reads entry o from diagonal |o| at row i (o >= 0) or at its mirror row i+o (o < 0), for o in O
+ * ascending -- its CSR order, with zeros where it has no entry (spmv_symdiag_kernel).  Rows with the same
+ * pattern id have the same offsets, so the patterns the covered rows use give O.
+ */
+_Static_assert(ACGB200_SYMDIAG_MAX == SLICE_MAXLEN, "mirrored diagonals hold the rows a slice may hold");
+
+int acgb200_symdiag_plan(int nrows, const struct acgb200_sliceplan *sp, const struct acgb200_patterns *pat,
+                         struct acgb200_symdiag *out)
+{
+    memset(out, 0, sizeof(*out));
+    if (!sp || sp->nslices <= 0 || !pat || !sp->patid) { out->reason = SYMDIAG_NO_SLICES; return ACG_SUCCESS; }
+    if (sp->nexc > 0) { out->reason = SYMDIAG_EXCEPTIONS; return ACG_SUCCESS; }
+    unsigned char *used = calloc((size_t) sp->npat + 1, 1);
+    if (!used) return ACG_ERR_ERRNO;
+    for (int s = 0; s < sp->nslices; s++)
+        for (int r = sp->slices[s].row0; r < sp->slices[s].row0 + sp->slices[s].nrows; r++) used[sp->patid[r]] = 1;
+    int no = 0;
+    for (int p = 0; p < sp->npat && !out->reason; p++) {
+        if (!used[p]) continue;
+        const int *off = pat->patoff + pat->patptr[p];
+        const int len = pat->patptr[p + 1] - pat->patptr[p];
+        for (int k = 0; k < len && !out->reason; k++) {
+            if (k > 0 && off[k] <= off[k - 1]) { out->reason = SYMDIAG_UNSORTED; break; }
+            int lo = 0;                                 /* insert off[k] into the sorted O */
+            while (lo < no && out->o[lo] < off[k]) lo++;
+            if (lo < no && out->o[lo] == off[k]) continue;
+            if (no == ACGB200_SYMDIAG_MAX) { out->reason = SYMDIAG_TOO_MANY; break; }
+            memmove(out->o + lo + 1, out->o + lo, (size_t) (no - lo) * sizeof(int));
+            out->o[lo] = off[k]; no++;
+        }
+    }
+    free(used);
+    if (out->reason) return ACG_SUCCESS;
+    out->no = no;
+    /* D: the absolute values, ascending (O is sorted, so merge its negative part reversed with the rest) */
+    int nd = 0, neg = 0;
+    while (neg < no && out->o[neg] < 0) neg++;
+    for (int a = neg - 1, b = neg; a >= 0 || b < no;) {
+        const int v = (b >= no || (a >= 0 && -out->o[a] <= out->o[b])) ? -out->o[a--] : out->o[b++];
+        if (nd == 0 || out->d[nd - 1] != v) out->d[nd++] = v;
+    }
+    out->nd = nd;
+    /* the stored diagonals replace the slice-major values: 8|D| bytes per covered row against 256 per block */
+    if ((int64_t) nd * sp->rows >= sp->blocks * 32) { out->reason = SYMDIAG_NO_GAIN; return ACG_SUCCESS; }
+    /* 32-bit value offsets in the kernel */
+    if ((int64_t) nd * ((int64_t) nrows + out->d[nd - 1] + 64) > INT32_MAX) out->reason = SYMDIAG_TOO_LARGE;
+    return ACG_SUCCESS;
+}
+
+/* Where the kernel finds entry e of a covered row i: diagonal d sits at [idx(d) * stride, + stride) with
+ * a[j, j+d] at margin + j; entry o is value voff + i and column i + coff (coff = o).  The margin and the
+ * stride are multiples of 32, so the reads of a slice's upper entries start on 256-byte boundaries. */
+void acgb200_symdiag_layout(int nrows, const struct acgb200_symdiag *sd, int *margin, int *stride,
+                            struct acgb200_symdiag_entry *tab)
+{
+    const int m = (sd->d[sd->nd - 1] + 31) & ~31;
+    *margin = m;
+    *stride = (m + nrows + 31) & ~31;
+    for (int e = 0; e < sd->no; e++) {
+        const int o = sd->o[e], a = o < 0 ? -o : o;
+        int idx = 0;
+        while (sd->d[idx] != a) idx++;
+        tab[e].voff = idx * *stride + m + (o < 0 ? o : 0);
+        tab[e].coff = o;
+    }
+}

@@ -18,7 +18,9 @@ extern "C" {
  * "spmv_nnz_cap", "spmv_rows_cap", "spmv_stages", "spmv_threads", "spmv_unroll",
  * "spmv_max_ctas" (SpMV tile plan overrides, read at acgsolvercuda_init), "spmv_slices"
  * (0/1, default 1: index-free slice-major storage of the rows that repeat a pattern, slices.c; shape
- * overrides "slice_ub", "slice_threads", "slice_max_ctas"), "spmv_merge" (-1/0/1,
+ * overrides "slice_ub", "slice_threads", "slice_max_ctas"), "spmv_symdiag" (1/0, default 1: the slice-covered rows
+ * of an exactly symmetric matrix read each stored value once -- the upper diagonals, every lower entry from its
+ * mirror row -- when the structure allows, slices.c; "symdiag_evict_first" 0/1 their L2 policy), "spmv_merge" (-1/0/1,
  * default -1: merge-path tiles when the row lengths are irregular, mergeplan.c; "merge_items", "merge_threads",
  * "merge_max_ctas"), "spmv_medium", "graph"
  * (0/1: replay iteration pairs as CUDA graphs), "redstream" (0/1: pipelined
@@ -128,6 +130,9 @@ struct acgb200_info {
     int spmv_merge_threads, spmv_merge_grid, spmv_merge_stages;    /* shape and grid of the merge-path kernel */
     int64_t spmv_slice_value_bytes;             /* slice-major values of the pattern slices, padding included */
     int64_t spmv_slice_nnz;                     /* nonzeros those slices cover (without padding) */
+    int spmv_symdiag_diagonals;                 /* upper diagonals stored for the slice-covered rows, whose lower entries
+                                                   come from their mirror rows (option "spmv_symdiag"); 0: off */
+    int64_t spmv_symdiag_bytes;                 /* their bytes, zero margins included */
 };
 ACG_API int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info);
 
@@ -151,6 +156,17 @@ ACG_API int acgb200_spmv_plan_host2(int nrows, const int64_t *rowptr, const int 
 ACG_API int acgb200_slices_host(int nrows, int cover_hi, const int64_t *rowptr, const int *colidx,
                                 int *slices4, int maxslices, unsigned char *covered, int64_t *totals6, int *spatoff,
                                 unsigned short *patid, int64_t *exc2);
+
+/* The mirrored-diagonal plan of the pattern slices of a 0-based CSR matrix (slices.c), host only: info5 gets
+ * {reason (0: eligible; 1 no slices, 2 exception rows, 3 a covered row not sorted, 4 more than 64 offsets,
+ * 5 no fewer bytes, 6 too large), |O|, |D|, zero margin, stride}, o the offsets O of the covered rows (64 ints),
+ * d the stored diagonals D (64 ints), tab2 {value offset, column offset} per entry of O (128 ints; eligible
+ * plans only): entry e of covered row i is value tab2[2e] + i of the diagonals -- diagonal D[k] at
+ * [k * stride, (k+1) * stride), a[j, j + D[k]] at margin + j -- times x[i + tab2[2e+1]].  acgsolvercuda_init
+ * uses the layout if this says eligible and the values pass a bitwise symmetry check on the device.  Rows
+ * [0,cover_hi) are eligible for slices. */
+ACG_API int acgb200_symdiag_host(int nrows, int cover_hi, const int64_t *rowptr, const int *colidx, int *info5,
+                                 int *o, int *d, int *tab2);
 
 /* acgsymcsrmatrix_dsymv_init (acg/symcsrmatrix.c:760-851) computed on the current CUDA device
  * (expand.cu): the packed triangle is uploaded, mirrored there into the full local block and the

@@ -22,7 +22,8 @@ import numpy as np          # noqa: E402
 
 DEFAULTS = dict(profile=0, spmv_lanes=0, spmv_nnz_cap=0, spmv_rows_cap=0, spmv_stages=0, spmv_threads=0,
                 spmv_unroll=0, spmv_max_ctas=0, graph=1, redstream=1, p2p=1, p2p_fuse=1, blas1_ctas=0, pdl=0,
-                spmv_medium=0, spmv_merge=-1, merge_items=0, merge_threads=0, merge_stages=0, merge_max_ctas=0, spmv_slices=1, slice_ub=0, slice_threads=0, slice_max_ctas=0)
+                spmv_medium=0, spmv_merge=-1, merge_items=0, merge_threads=0, merge_stages=0, merge_max_ctas=0, spmv_slices=1, slice_ub=0, slice_threads=0, slice_max_ctas=0,
+                spmv_symdiag=1, symdiag_evict_first=0)
 
 VARIANTS = {
     "base": {},
@@ -42,6 +43,11 @@ VARIANTS = {
     "s9": {"slice_ub": 9}, "s8": {"slice_ub": 8}, "s7": {"slice_ub": 7}, "s5": {"slice_ub": 5},
     "s9_t256": {"slice_ub": 9, "slice_threads": 256}, "s7_t256": {"slice_ub": 7, "slice_threads": 256},
     "s9_c8": {"slice_ub": 9, "slice_max_ctas": 8},
+    # mirrored diagonals (option spmv_symdiag): off (the slice kernel), their values evict-first in L2, and
+    # resident CTAs per SM, which sets how far the grid-stride front runs ahead of the mirror reads
+    "nosymdiag": {"spmv_symdiag": 0},
+    "sd_ef": {"symdiag_evict_first": 1},
+    "sd_c4": {"slice_max_ctas": 4}, "sd_c8": {"slice_max_ctas": 8},
 }
 
 
