@@ -62,9 +62,12 @@ static struct {
     int slice_ub, slice_threads, slice_max_ctas;   /* slice kernel shape overrides (0 = default) */
     int spmv_symdiag;   /* 1: mirrored diagonals for the slice-covered rows when the matrix allows (slices.c), 0: off */
     int symdiag_evict_first;   /* 1: L2 evict-first policy on the stored diagonals (A/B; the default reuses them in L2) */
+    int pcg_fused;      /* 1: pipelined CG runs each iteration's product and update in one kernel where the plan allows
+                         * (one GPU, mirrored diagonals; DESIGN.md section 4a), 0: off (A/B) */
+    int pcg_evict_first;   /* 1: L2 evict-first policy on the fused kernel's vector streams (A/B) */
     int loaded;
 } cfg = { .check_every = 8, .graph = 1, .redstream = 1, .p2p = 1, .p2p_fuse = 1, .spmv_slices = 1, .spmv_merge = -1,
-          .spmv_symdiag = 1 };
+          .spmv_symdiag = 1, .pcg_fused = 1, .pcg_evict_first = 1 };
 
 static void cfg_load(void)
 {
@@ -99,6 +102,8 @@ static void cfg_load(void)
     if ((s = getenv("ACGB200_SLICE_MAX_CTAS"))) cfg.slice_max_ctas = atoi(s);
     if ((s = getenv("ACGB200_SPMV_SYMDIAG"))) cfg.spmv_symdiag = atoi(s);
     if ((s = getenv("ACGB200_SYMDIAG_EVICT_FIRST"))) cfg.symdiag_evict_first = atoi(s);
+    if ((s = getenv("ACGB200_PCG_FUSED"))) cfg.pcg_fused = atoi(s);
+    if ((s = getenv("ACGB200_PCG_EVICT_FIRST"))) cfg.pcg_evict_first = atoi(s);
     acgb200_blas1_set_ctas_per_sm(cfg.blas1_ctas);
     acgb200_set_pdl(cfg.pdl);
 }
@@ -133,6 +138,8 @@ int acgb200_set_option(const char *key, int value)
     else if (!strcmp(key, "slice_max_ctas")) cfg.slice_max_ctas = value;
     else if (!strcmp(key, "spmv_symdiag")) cfg.spmv_symdiag = value;
     else if (!strcmp(key, "symdiag_evict_first")) cfg.symdiag_evict_first = value;
+    else if (!strcmp(key, "pcg_fused")) cfg.pcg_fused = value;
+    else if (!strcmp(key, "pcg_evict_first")) cfg.pcg_evict_first = value;
     else return ACG_ERR_INVALID_VALUE;
     return ACG_SUCCESS;
 }
@@ -172,6 +179,8 @@ struct priv {
     double last_spmv_ms;                /* profiled SpMV time of the last solve */
     double last_blas_ms;                /* profiled fused-update time of the last solve */
     int last_spmv_n;
+    int last_fused;                     /* the last solve ran the fused pipelined-CG iteration */
+    double *d_w2;                       /* fused pipelined CG: the second buffer of w (made at the first such solve) */
     int commsize;                       /* ranks of the communicator given to acgsolvercuda_init */
     /* several right-hand sides (acgsolvercuda_solve_multi), made at the first multi-vector call */
     struct acgb200_mstate *d_ms, *h_ms; /* per-column scalars on the device / pinned staging */
@@ -280,7 +289,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
         if (pv->commstream) cudaStreamDestroy(pv->commstream);
         if (pv->redstream) cudaStreamDestroy(pv->redstream);
         if (pv->ev_red) cudaEventDestroy(pv->ev_red);
-        cudaFree(pv->d_b); cudaFree(pv->d_x);
+        cudaFree(pv->d_b); cudaFree(pv->d_x); cudaFree(pv->d_w2);
         cudaFree(pv->d_ms); cudaFreeHost(pv->h_ms); cudaFree(pv->d_ranges);
         cudaFree(pv->d_ss); cudaFreeHost(pv->h_ss);
         cudaFree(pv->d_mx); cudaFree(pv->d_mb); cudaFree(pv->d_mr); cudaFree(pv->d_mp); cudaFree(pv->d_mt);
@@ -851,6 +860,9 @@ struct solvectx {
     int p2p;                  /* loop exchanges go through peer memory */
     int mk;                   /* multi-vector loop: block width K (0: single vector) */
     int shifted;              /* shifted-systems loop (acgsolvercuda_solve_shifted) */
+    int fused;                /* pipelined loop: one fused iteration (acgb200_pcg_fused_launch); its control word
+                               * alternates between ctrl[0] and ctrl[1] by iteration parity */
+    int issued;               /* iterations iterate() issued, inactive ones included */
 };
 
 static int evpool_reserve(struct evpool *p, int n)
@@ -1089,7 +1101,8 @@ static double threshold(double atol, double rtol, double r0nrm2)
 static int graph_signature(const struct solvectx *c)
 {
     return 1 | (c->multi ? 2 : 0) | (c->p2p ? 4 : 0) | (c->pv->p2p.h_desc.fuse ? 8 : 0) | (cfg.pdl ? 16 : 0)
-           | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0) | (c->shifted ? 128 : 0) | (c->mk << 8);
+           | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0) | (c->shifted ? 128 : 0) | (c->mk << 8)
+           | (c->fused ? 1 << 16 : 0);
 }
 
 static int capture_pair(struct solvectx *c, int kind, int (*issue)(struct solvectx *, int))
@@ -1143,7 +1156,7 @@ static int iterate(struct solvectx *c, int maxits, int poll, int kind, int (*iss
         }
         if (!poll || (since_poll < cfg.check_every && issued < maxits)) continue;
         since_poll = 0;
-        CU(cudaMemcpyAsync(&pv->h_ctrl[slot], &pv->d_st->ctrl[0], sizeof(struct acgb200_ctrl),
+        CU(cudaMemcpyAsync(&pv->h_ctrl[slot], &pv->d_st->ctrl[c->fused ? issued & 1 : 0], sizeof(struct acgb200_ctrl),
                            cudaMemcpyDeviceToHost, pv->stream));
         CU(cudaEventRecord(pv->ev_poll[slot], pv->stream));
         if (have_prev) {
@@ -1152,6 +1165,7 @@ static int iterate(struct solvectx *c, int maxits, int poll, int kind, int (*iss
         }
         have_prev = 1; slot ^= 1;
     }
+    c->issued = issued;
     CU(cudaStreamSynchronize(pv->stream));
     if (c->multi) { CU(cudaStreamSynchronize(pv->commstream)); CU(cudaStreamSynchronize(pv->redstream)); }
     if (c->multi && c->p2p) {
@@ -1230,6 +1244,7 @@ int acgsolvercuda_solvempi(
     struct acgb200_devstate h;
 
     c.p2p = c.multi && pv->p2p.enabled && cfg.p2p;
+    pv->last_fused = 0;
     /* a rank that is ahead must not store into a peer's window while that peer's kernels of the
      * previous solve are still reading it: order the first post of this solve behind every rank */
     if (c.p2p) OK(acgcomm_barrier(pv->stream, comm, errcode));
@@ -1854,6 +1869,21 @@ static int pipelined_iteration(struct solvectx *c, int k)
     int *errcode = c->errcode;
     const int s = k & 1, n = pv->nowned;
     const int peer = c->multi && c->p2p;
+    if (c->fused) {
+        /* one GPU: iteration k gathers w from buffer k&1 and writes w_{k+1} into the other (DESIGN.md section 4a) */
+        struct acgb200_pcgargs a;
+        memset(&a, 0, sizeof(a));
+        a.plan = &pv->plan; a.rowptr = cg->d_rowptr; a.colidx = cg->d_colidx; a.a = cg->d_a;
+        a.w = s ? pv->d_w2 : cg->d_w; a.w_next = s ? cg->d_w : pv->d_w2;
+        a.q = cg->d_q; a.z = cg->d_z; a.t = cg->d_t; a.p = cg->d_p; a.r = cg->d_r; a.x = c->d_x;
+        a.st = st; a.cin = s; a.vec_evict_first = cfg.pcg_evict_first;
+        /* the whole iteration is timed as the product: no separate update time on this path */
+        prof_mark(c, &pv->gemv);
+        KL(acgb200_pcg_fused_launch(&a, pv->stream));
+        prof_mark(c, &pv->gemv);
+        c->launches += 1 + (pv->plan.ntiles > 0 ? 2 : 0);
+        return ACG_SUCCESS;
+    }
     /* One allreduce for {gamma,delta} (acg/cgcuda.c:1697).  The reference
      * issues it on the compute stream ahead of q = A w, i.e. serialised.  Here:
      * peer-memory mode -- the partials were pushed to every rank right after
@@ -1910,6 +1940,15 @@ int acgsolvercuda_solve_pipelined(
     OK(ensure_vec(&cg->z, &cg->d_z, A, pv->nvec, errcode));
 
     c.p2p = c.multi && pv->p2p.enabled && cfg.p2p;
+    /* one kernel per iteration: one GPU, mirrored diagonals for the slice rows, all other rows in tiles */
+    const struct acgb200_spmvplan *pl = &pv->plan;
+    c.fused = cfg.pcg_fused && !c.multi && pv->nghost == 0 && pv->nborder == 0 && pl->symdiag_nd > 0 && pl->pcg_grid > 0
+              && pl->nmtiles == 0 && pl->nmed == 0 && pl->nlong == 0;
+    pv->last_fused = c.fused;
+    if (c.fused && !pv->d_w2) {
+        CU(cudaMalloc((void **) &pv->d_w2, ((size_t) pv->nvec + 2) * sizeof(double)));
+        CU(cudaMemsetAsync(pv->d_w2, 0, ((size_t) pv->nvec + 2) * sizeof(double), pv->stream));
+    }
     if (c.p2p) OK(acgcomm_barrier(pv->stream, comm, errcode));     /* as in acgsolvercuda_solvempi */
     if (warmup > 0) {
         memset(&h, 0, sizeof(h));
@@ -1982,12 +2021,14 @@ int acgsolvercuda_solve_pipelined(
         }
         OK(iterate(&c, maxits, tol > 0, 1, pipelined_iteration));
         OK(pull_state(&c, &h));
-        cg->niterations = h.ctrl[0].iter;
-        converged = h.ctrl[0].done;
+        const struct acgb200_ctrl cw = h.ctrl[c.fused ? c.issued & 1 : 0];
+        cg->niterations = cw.iter;
+        converged = cw.done;
         /* the reference reports sqrt(gamma) of the last *tested* iterate
          * (acg/cgcuda.c:1760): gamma_k at convergence, gamma_{maxits-1} otherwise */
         const int kk = converged ? cg->niterations : (cg->niterations > 0 ? cg->niterations - 1 : 0);
-        const double g = converged ? h.final_rr : (kk == 0 ? gd0[0] : (c.multi ? h.gd[kk & 1][0] : h.gd_loc[kk & 1][0]));
+        const double g = converged ? h.final_rr
+            : (kk == 0 ? gd0[0] : (c.multi ? h.gd[kk & 1][0] : h.gd_loc[c.fused ? kk % 3 : kk & 1][0]));
         cg->rnrm2 = sqrt(g);
         cg->ntotaliterations += cg->niterations;
     }
@@ -2385,10 +2426,13 @@ int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info
     info->spmv_slice_threads = pv->plan.slice_threads;
     info->spmv_merge_threads = pv->plan.merge_threads; info->spmv_merge_grid = pv->plan.merge_grid;
     info->spmv_merge_stages = pv->plan.merge_stages;
-    info->spmv_min_bytes = acgb200_spmv_min_bytes(&pv->plan);
+    /* the bytes of what profile mode times as one product: the whole iteration on the fused path */
+    info->spmv_min_bytes = pv->last_fused ? acgb200_pcg_iteration_min_bytes(&pv->plan) : acgb200_spmv_min_bytes(&pv->plan);
     info->spmv_slice_value_bytes = pv->plan.nslices > 0 ? pv->plan.sval_blocks * 32 * (int64_t) sizeof(double) : 0;
     info->spmv_slice_nnz = pv->plan.nslices > 0 ? pv->plan.slice_nnz : 0;
     info->spmv_symdiag_diagonals = pv->plan.symdiag_nd;
     info->spmv_symdiag_bytes = (int64_t) pv->plan.symdiag_nd * pv->plan.symdiag_stride * (int64_t) sizeof(double);
+    info->pcg_fused = pv->last_fused;
+    info->pcg_fused_min_bytes = pv->plan.symdiag_nd > 0 ? acgb200_pcg_fused_min_bytes(&pv->plan) : 0;
     return ACG_SUCCESS;
 }

@@ -89,6 +89,7 @@ struct acgb200_spmvplan {
     double *d_hval;                  /* [symdiag_nd * symdiag_stride] */
     const int *symdiag_colidx;       /* device CSR columns the fill reads (borrowed, valid during init only) */
     int *d_symdiag_bad;              /* fill-time symmetry check: 0 passed (written by acgb200_slices_fill) */
+    int pcg_grid;                    /* grid of the fused pipelined-CG kernel (acgb200_pcg_fused_launch); 0: none */
     /* merge-path tiles (mergeplan.c): rows [0, merge_rows) of an irregular (power-law) matrix, cut into tiles
      * of merge_items merged items (row ends + nonzeros) and multiplied by spmv_merge_kernel; rows cut by tile
      * boundaries are finished by spmv_merge_fix_kernel from the tiles' partial sums */
@@ -196,8 +197,10 @@ struct acgb200_devstate {
     /* classic CG: slot = iteration parity */
     double pap_loc[2], pap[2];       /* local partial / global (p,Ap) */
     double rr_loc[2], rr[2];         /* (r_k,r_k) lives in slot k&1 */
-    /* pipelined CG */
-    double gd_loc[2][2], gd[2][2];   /* {gamma,delta} = {(r,r),(w,r)} */
+    /* pipelined CG: {gamma,delta} = {(r,r),(w,r)}.  gd_loc is indexed by parity (slots 0, 1) on the two-kernel
+     * path, and on the fused path as a ring of three: iteration k reads slot k%3, adds into (k+1)%3 and
+     * zeroes (k+2)%3, so its last kernel never adds into a slot it zeroes (DESIGN.md section 4a) */
+    double gd_loc[3][2], gd[2][2];
     double prev[2][2];               /* {gamma_{k-1}, alpha_{k-1}} read by update k from slot k&1 */
     /* setup-time reductions */
     double tmp_loc[2], tmp[2];
@@ -333,6 +336,34 @@ int acgb200_pcg_update(int n, struct acgb200_devstate *st, int cin, int cout, in
                        const double *q, double *z, double *w, double *t, double *p,
                        double *r, double *x, cudaStream_t stream);
 
+/* One whole pipelined-CG iteration on one GPU for a plan with mirrored diagonals and no merge tiles, medium
+ * or long rows: the covered rows' product and update in one kernel (spmv_symdiag_kernel with its PCG
+ * epilogue), which reads the control word ctrl[cin] and writes ctrl[cin ^ 1].  With tiles, the tile kernel
+ * (q = A w over the other rows) and their update run first and pass the word through ctrl[2] and ctrl[3].
+ * w is read, w_{k+1} goes to w_next (another buffer: other rows still gather w); z, t, p, r, x in place. */
+struct acgb200_pcgargs {
+    const struct acgb200_spmvplan *plan;
+    const int *rowptr, *colidx; const double *a;    /* CSR of the tile rows */
+    const double *w; double *w_next;
+    double *q;                                      /* the tile rows' product */
+    double *z, *t, *p, *r, *x;
+    struct acgb200_devstate *st;
+    int cin;                                        /* 0 or 1: the iteration's parity */
+    int vec_evict_first;                            /* L2 policy of the fused kernel's vector streams */
+};
+/* Weak in the host code, like the multi-vector launchers below: the host-logic test build of tests/hostsim
+ * never plans mirrored diagonals, so it never selects this path and need not define it. */
+#if defined(__CUDACC__)
+#define ACGB200_MULTI_LAUNCHER
+#else
+#define ACGB200_MULTI_LAUNCHER __attribute__((weak))
+#endif
+ACGB200_MULTI_LAUNCHER int acgb200_pcg_fused_launch(const struct acgb200_pcgargs *a, cudaStream_t stream);
+/* the bytes the fused launch moves at least (8 |D| + 96 per covered row), and those of the whole fused
+ * iteration (the tile kernel's bytes and 104 per tile row for their update on top) */
+int64_t acgb200_pcg_fused_min_bytes(const struct acgb200_spmvplan *plan);
+int64_t acgb200_pcg_iteration_min_bytes(const struct acgb200_spmvplan *plan);
+
 /* the reference's public BLAS-1 building blocks (acg/cg-kernels-cuda.h:45-97; cgcuda.c wraps them) */
 int acgb200_helper_axpy(int op, int n, const double *num, const double *den, const double *x, double *y, cudaStream_t stream);
 int acgb200_helper_scalars(int op, double *out0, double *out1, const double *num, const double *den, cudaStream_t stream);
@@ -400,11 +431,6 @@ struct acgb200_spmmargs {
  * single-vector kernels only -- the host-logic test build of tests/hostsim -- still loads, and
  * acgsolvercuda_solve_multi / acgsolvercuda_spmm_mode return ACG_ERR_NOT_SUPPORTED there (no other path
  * runs instead).  libacgb200.so always defines them (kernels.cu). */
-#if defined(__CUDACC__)
-#define ACGB200_MULTI_LAUNCHER
-#else
-#define ACGB200_MULTI_LAUNCHER __attribute__((weak))
-#endif
 ACGB200_MULTI_LAUNCHER int acgb200_spmm_launch(const struct acgb200_spmmargs *a, cudaStream_t stream);
 /* classic CG updates with per-column alpha_j, beta_j; columns outside the incoming mask are left alone */
 ACGB200_MULTI_LAUNCHER int acgb200_cg_multi_update_r(int n, int k, struct acgb200_devstate *st, struct acgb200_mstate *ms, int cin, int cout,

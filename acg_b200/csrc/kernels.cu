@@ -121,6 +121,20 @@ __device__ __forceinline__ double ld_stream(const double *p, uint64_t pol)
     return v;
 }
 
+/* a vector entry read once and written back by the same thread in the same kernel (the fused pipelined-CG
+ * update): the coherent path, no L1 line, the caller's L2 policy */
+__device__ __forceinline__ double ld_vec(const double *p, uint64_t pol)
+{
+    double v;
+    asm volatile("ld.global.L1::no_allocate.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(v) : "l"(p), "l"(pol));
+    return v;
+}
+
+__device__ __forceinline__ void st_vec(double *p, double v, uint64_t pol)
+{
+    asm volatile("st.global.L2::cache_hint.f64 [%0], %1, %2;" :: "l"(p), "d"(v), "l"(pol) : "memory");
+}
+
 /* Programmatic dependent launch (opt-in, ACGB200_PDL=1).  Every kernel of the
  * iteration chain starts with this: wait until the preceding kernel of the
  * stream has completed and flushed (nothing in global memory is touched before),
@@ -183,6 +197,45 @@ __device__ __forceinline__ Gate gate_read(const acgb200_ctrl *cin, const acgb200
         g.active = (c.y == 0) && (c.x < st->maxits);
     }
     return g;
+}
+
+/* The scalars of pipelined-CG update k on the fused path (one GPU): {gamma_k, delta_k} from accumulator ring
+ * slot k % 3, the expressions of pcg_update_kernel.  Every kernel of the iteration computes them alike. */
+struct PcgStep { double gamma, alpha, beta; bool conv; };
+
+__device__ __forceinline__ PcgStep pcg_step(const acgb200_devstate *st, int iter)
+{
+    PcgStep o;
+    const int s = iter & 1, slot = iter % 3;
+    const double gamma = st->gd_loc[slot][0], delta = st->gd_loc[slot][1];
+    const double gamma_prev = st->prev[s][0], alpha_prev = st->prev[s][1];
+    o.gamma = gamma;
+    o.conv = st->tol > 0.0 && sqrt(gamma) < st->tol;
+    o.beta = gamma / gamma_prev;
+    o.alpha = gamma / (delta - o.beta * gamma / alpha_prev);
+    return o;
+}
+
+/* z=q+beta z; t=w+beta t; p=r+beta p; x+=alpha p; r-=alpha t; w'=w-alpha z for row i (the fma chain of
+ * pcg_update_kernel), w' into the other buffer; gamma'=(r,r), delta'=(w',r) accumulate in g2, d2 */
+__device__ __forceinline__ void pcg_row(int i, double qi, double wi, const PcgStep &k, double *__restrict__ z,
+                                        double *__restrict__ t, double *__restrict__ p, double *__restrict__ r,
+                                        double *__restrict__ x, double *__restrict__ w_next, uint64_t pol,
+                                        double &g2, double &d2)
+{
+    const double zi = ld_vec(z + i, pol), ti = ld_vec(t + i, pol), pi = ld_vec(p + i, pol);
+    const double ri = ld_vec(r + i, pol), xi = ld_vec(x + i, pol);
+    const double zv = fma(k.beta, zi, qi);
+    const double tv = fma(k.beta, ti, wi);
+    const double pv = fma(k.beta, pi, ri);
+    const double rv = fma(-k.alpha, tv, ri);
+    const double wv = fma(-k.alpha, zv, wi);
+    st_vec(z + i, zv, pol); st_vec(t + i, tv, pol); st_vec(p + i, pv, pol);
+    st_vec(x + i, fma(k.alpha, pv, xi), pol);
+    st_vec(r + i, rv, pol);
+    st_vec(w_next + i, wv, pol);
+    g2 = fma(rv, rv, g2);
+    d2 = fma(wv, rv, d2);
 }
 
 /* ------------------------------------------------------------------------ */
@@ -729,6 +782,9 @@ struct SymdiagParams {
     acgb200_ctrl *ctrl_out;
     acgb200_devstate *st;
     int housekeeping;
+    /* pipelined-CG epilogue (PCG): x above is w_k; z, t, p, r, xs updated in place, w_{k+1} into w_next */
+    double *z, *t, *p, *r, *xs, *w_next;
+    int vec_evict_first;
 };
 
 /*
@@ -743,9 +799,14 @@ struct SymdiagParams {
  * accumulator; an offset the row does not have contributes fma(0, x[col], sum) == sum.  One difference
  * follows: such a slot gathers x at its (clamped) column where the slice kernel's padding gathers x[row],
  * so a non-finite x there makes the row NaN (0 * Inf) where the slice kernel may not.
+ *
+ * PCG: the whole pipelined-CG iteration k for the covered rows (DESIGN section 4a).  The row's sum is q_i
+ * and goes straight into the update (pcg_row) instead of to memory; the kernel is the iteration's last, so
+ * block 0 advances the control word and zeroes ring slot (k+2) % 3 while every CTA adds into (k+1) % 3.
+ * A met convergence test returns before the product.  At most 40 registers: 12 CTAs of 128 threads.
  */
-template <int UB, int T>
-__global__ void __launch_bounds__(T)
+template <int UB, int T, bool PCG>
+__global__ void __launch_bounds__(T, PCG ? 1536 / T : 0)
 spmv_symdiag_kernel(const SymdiagParams P)
 {
     __shared__ int2 tab_s[ACGB200_SYMDIAG_MAX];
@@ -753,7 +814,21 @@ spmv_symdiag_kernel(const SymdiagParams P)
     const int tid = threadIdx.x;
     pdl_prologue();
     const Gate gate = gate_read(P.ctrl_in, P.st);
-    if (P.ctrl_out && blockIdx.x == 0 && tid == 0 && P.ctrl_in) {
+    PcgStep k;
+    if (PCG) {
+        k = pcg_step(P.st, gate.iter);
+        if (blockIdx.x == 0 && tid == 0) {
+            acgb200_ctrl c = *P.ctrl_in;
+            if (gate.active) {
+                const int s = gate.iter & 1, z = (gate.iter + 2) % 3;
+                P.st->gd_loc[z][0] = 0.0; P.st->gd_loc[z][1] = 0.0;
+                if (k.conv) { c.done = 1; P.st->final_rr = k.gamma; }
+                else { c.iter = gate.iter + 1; P.st->prev[s ^ 1][0] = k.gamma; P.st->prev[s ^ 1][1] = k.alpha; }
+            }
+            *P.ctrl_out = c;
+        }
+        if (!gate.active || k.conv) return;
+    } else if (P.ctrl_out && blockIdx.x == 0 && tid == 0 && P.ctrl_in) {
         *P.ctrl_out = *P.ctrl_in;
         if (gate.active) {
             const int s = gate.iter & 1;
@@ -772,7 +847,9 @@ spmv_symdiag_kernel(const SymdiagParams P)
     const int nwarps = (gridDim.x * T) >> 5;
     const int cmax = P.nrows - 1;
     const int L = P.no;
-    double dot = 0.0;
+    double dot = 0.0, dot2 = 0.0;
+    /* the vector streams of the update pass through L2 once: see the measurements in DESIGN section 4a */
+    const uint64_t vpol = PCG ? (P.vec_evict_first ? l2_policy_evict_first() : l2_policy_evict_normal()) : 0;
     for (int s = warp; s < P.nslices; s += nwarps) {
         const int row = __ldg(&P.slices[s].row0) + lane;
         const double *hv = P.hval + row;
@@ -796,7 +873,10 @@ spmv_symdiag_kernel(const SymdiagParams P)
 #pragma unroll
             for (int u = 0; u < UB; u++) if (e + u < L) sum = fma(vv[u], xv[u], sum);
         }
-        if (P.mode == SPMV_R_B_AX) {
+        if (PCG) {
+            /* w_i was gathered by this row a moment ago: an L1 hit, not a third stream */
+            pcg_row(row, sum, __ldg(P.x + row), k, P.z, P.t, P.p, P.r, P.xs, P.w_next, vpol, dot, dot2);
+        } else if (P.mode == SPMV_R_B_AX) {
             const double r = P.b[row] - sum;
             P.y[row] = r;
             if (row < P.dotrows) dot = fma(r, r, dot);
@@ -805,7 +885,15 @@ spmv_symdiag_kernel(const SymdiagParams P)
             if (P.mode == SPMV_Y_AX_DOT && row < P.dotrows) dot = fma(__ldg(P.x + row), sum, dot);
         }
     }
-    if (P.acc) {
+    if (PCG) {
+        dot = block_sum(dot, red);
+        dot2 = block_sum(dot2, red);
+        if (tid == 0) {
+            double *acc = P.st->gd_loc[(gate.iter + 1) % 3];
+            atomicAdd(&acc[0], dot);
+            atomicAdd(&acc[1], dot2);
+        }
+    } else if (P.acc) {
         const double v = block_sum(dot, red);
         if (tid == 0 && v != 0.0) atomicAdd(P.acc, v);
     }
@@ -1434,6 +1522,39 @@ pcg_update_kernel(int n, acgb200_devstate *st, int cin, int cout, int multi, acg
             p2p_publish_red(P, 0, s ^ 1, P->rbase + it1, &st->gd_loc[s ^ 1][0], 2);
             p2p_publish_halo(P, P->hbase + it1);
         }
+    }
+}
+
+/* Fused pipelined CG, rows outside the slices: the update of the tile rows from the tile kernel's q, the
+ * row ranges of the tile plan, one CTA per tile and trip.  Adds into the same ring slot as the fused kernel,
+ * which runs after it and advances the control word; this one only forwards it. */
+#define PCG_TAIL_THREADS 128
+__global__ void __launch_bounds__(PCG_TAIL_THREADS)
+pcg_tail_update_kernel(const acgb200_tile *__restrict__ tiles, int ntiles, acgb200_devstate *st,
+                       const acgb200_ctrl *cin, acgb200_ctrl *cout, const double *__restrict__ q,
+                       const double *__restrict__ w, double *__restrict__ w_next, double *__restrict__ z,
+                       double *__restrict__ t, double *__restrict__ p, double *__restrict__ r, double *__restrict__ x)
+{
+    __shared__ double red[PCG_TAIL_THREADS / 32];
+    pdl_prologue();
+    const Gate g = gate_read(cin, st);
+    if (blockIdx.x == 0 && threadIdx.x == 0) *cout = *cin;
+    if (!g.active) return;
+    const PcgStep k = pcg_step(st, g.iter);
+    if (k.conv) return;
+    const uint64_t pol = l2_policy_evict_normal();
+    double g2 = 0.0, d2 = 0.0;
+    for (int b = blockIdx.x; b < ntiles; b += gridDim.x) {
+        const acgb200_tile tl = tiles[b];
+        for (int i = tl.row_begin + (int) threadIdx.x; i < tl.row_begin + tl.nrows; i += PCG_TAIL_THREADS)
+            pcg_row(i, q[i], w[i], k, z, t, p, r, x, w_next, pol, g2, d2);
+    }
+    g2 = block_sum(g2, red);
+    d2 = block_sum(d2, red);
+    if (threadIdx.x == 0) {
+        double *acc = st->gd_loc[(g.iter + 1) % 3];
+        atomicAdd(&acc[0], g2);
+        atomicAdd(&acc[1], d2);
     }
 }
 
@@ -2082,10 +2203,11 @@ static slice_fn slice_variant(int UB, int T, int EXC)
 
 typedef void (*symdiag_fn)(const SymdiagParams);
 
-/* the mirrored-diagonal kernel for exactly the (UB, T) pairs of slice_variant */
-static symdiag_fn symdiag_variant(int UB, int T)
+/* the mirrored-diagonal kernel for exactly the (UB, T) pairs of slice_variant; pcg: with the fused
+ * pipelined-CG epilogue */
+static symdiag_fn symdiag_variant(int UB, int T, bool pcg)
 {
-#define X(u, t) if (UB == u && T == t) return spmv_symdiag_kernel<u, t>;
+#define X(u, t) if (UB == u && T == t) return pcg ? spmv_symdiag_kernel<u, t, true> : spmv_symdiag_kernel<u, t, false>;
     X(5, 128) X(7, 128) X(8, 128) X(9, 128) X(7, 256) X(8, 256) X(9, 256)
 #undef X
     return NULL;
@@ -2139,7 +2261,7 @@ extern "C" int acgb200_spmv_configure(acgb200_spmvplan *pl)
     }
     if (pl->nslices > 0) {
         /* the mirrored-diagonal kernel, when the plan has them, takes the slice kernel's place and grid rule */
-        const void *sfn = pl->symdiag_nd > 0 ? (const void *) symdiag_variant(pl->slice_ub, pl->slice_threads)
+        const void *sfn = pl->symdiag_nd > 0 ? (const void *) symdiag_variant(pl->slice_ub, pl->slice_threads, false)
                                              : (const void *) slice_variant(pl->slice_ub, pl->slice_threads, pl->slice_exc > 0);
         if (!sfn) return (int) cudaErrorInvalidConfiguration;
         pl->slice_smem = pl->symdiag_nd > 0 ? 0 : ((pl->slice_npat * pl->slice_lpad + 3) & ~3) * (int) sizeof(int);
@@ -2156,7 +2278,9 @@ extern "C" int acgb200_spmv_configure(acgb200_spmvplan *pl)
              * mirror distance, and its rows' bytes (8 |D| + 16 per row) are what passes through L2 between the
              * two reads: keep them within half of the L2.  C3 (14 diagonals): 12 of the 16 CTAs of 128
              * threads the registers allow, 1026-1029 it/s against 937-939 with 16 (H100 SXM, 400 W, DESIGN
-             * section 3a); C2 (4 diagonals) stays at 16. */
+             * section 3a); C2 (4 diagonals) stays at 16.  The fused pipelined-CG kernel moves 80 more bytes per
+             * row, all evict-first; with it C3 ran at 1154 (8), 1217 (10), 1204 (12), 1204 (16) it/s, so the
+             * rule stands (DESIGN section 4a). */
             int dev = 0, l2 = 0;
             if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev) == cudaSuccess && l2 > 0) {
                 const long long row_bytes = 8LL * pl->symdiag_nd + 16;
@@ -2169,6 +2293,16 @@ extern "C" int acgb200_spmv_configure(acgb200_spmvplan *pl)
         const long long need = ((long long) pl->nslices * 32 + pl->slice_threads - 1) / pl->slice_threads;
         if (sgrid > need) sgrid = need;
         pl->slice_grid = (int) (sgrid < 1 ? 1 : sgrid);
+        pl->pcg_grid = 0;
+        if (pl->symdiag_nd > 0) {
+            /* the fused pipelined-CG kernel: the same grid, unless its registers allow fewer CTAs */
+            int fper = 0;
+            err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fper, (const void *) symdiag_variant(pl->slice_ub, pl->slice_threads, true),
+                                                                pl->slice_threads, 0);
+            if (err) return (int) err;
+            const long long fgrid = (long long) acgb200_num_sms() * (fper < 1 ? 1 : fper);
+            pl->pcg_grid = (int) (fgrid < pl->slice_grid ? fgrid : pl->slice_grid);
+        }
     }
     return 0;
 }
@@ -2197,6 +2331,24 @@ extern "C" int acgb200_slices_fill(const acgb200_spmvplan *pl, const int *d_rowp
     symdiag_fill_kernel<<<(int) (fgrid < 1 ? 1 : fgrid), 256, 0, stream>>>(pl->nrows, d_rowptr, pl->symdiag_colidx, d_a, pl->d_hval,
                                                                           pl->symdiag_nd, D, pl->symdiag_stride, pl->symdiag_margin);
     symdiag_check_kernel<<<(int) grid, 256, 0, stream>>>(S, d_rowptr, pl->symdiag_colidx, d_a, pl->d_symdiag_bad);
+    return (int) cudaGetLastError();
+}
+
+/* the tile kernel over the plan's tiles */
+static int launch_tiles(const acgb200_spmvargs *a, cudaStream_t stream)
+{
+    const acgb200_spmvplan *pl = a->plan;
+    SpmvParams P;
+    P.tiles = pl->d_tiles; P.ntiles = pl->ntiles;
+    P.sc = stage_slots(pl); P.stage_bytes = stage_bytes(pl); P.nstages = pl->nstages;
+    P.rowptr = a->rowptr; P.colidx = a->colidx; P.a = a->a; P.x = a->x; P.y = a->y; P.b = a->b;
+    P.acc = a->acc; P.dotrows = a->dotrows; P.mode = a->mode;
+    P.ctrl_in = a->ctrl_in; P.ctrl_out = a->ctrl_out; P.st = a->st; P.housekeeping = a->housekeeping;
+    P.p2p = (acgb200_p2pdev *) a->p2p; P.od_rowoffset = a->od_rowoffset; P.od_nrows = a->od_nrows;
+    P.orowptr = a->orowptr; P.ocolidx = a->ocolidx; P.oa = a->oa; P.pub_ch = a->p2p ? a->pub_ch : -1;
+    const cudaError_t le = launch_chain(spmv_variant(pl->lanes_per_row, pl->threads, pl->unroll),
+                                        pl->grid, pl->threads, (size_t) pl->smem_bytes, stream, P);
+    if (le) return (int) le;
     return (int) cudaGetLastError();
 }
 
@@ -2235,7 +2387,7 @@ extern "C" int acgb200_spmv_launch(const acgb200_spmvargs *a, cudaStream_t strea
         memcpy(S.tab, pl->symdiag_tab, sizeof(S.tab));
         S.x = a->x; S.y = a->y; S.b = a->b; S.acc = a->acc; S.dotrows = a->dotrows; S.mode = a->mode;
         S.ctrl_in = a->ctrl_in; S.ctrl_out = slices_forward ? a->ctrl_out : NULL; S.st = a->st; S.housekeeping = a->housekeeping;
-        const cudaError_t le = launch_chain(symdiag_variant(pl->slice_ub, pl->slice_threads), pl->slice_grid, pl->slice_threads,
+        const cudaError_t le = launch_chain(symdiag_variant(pl->slice_ub, pl->slice_threads, false), pl->slice_grid, pl->slice_threads,
                                             (size_t) 0, stream, S);
         if (le) return (int) le;
     } else if (pl->nslices > 0) {
@@ -2251,19 +2403,8 @@ extern "C" int acgb200_spmv_launch(const acgb200_spmvargs *a, cudaStream_t strea
         if (le) return (int) le;
     }
     if (pl->ntiles > 0 || (a->ctrl_in && !slices_forward)) {   /* with no tiles the kernel still forwards the control word */
-        SpmvParams P;
-        P.tiles = pl->d_tiles; P.ntiles = pl->ntiles;
-        P.sc = stage_slots(pl); P.stage_bytes = stage_bytes(pl); P.nstages = pl->nstages;
-        P.rowptr = a->rowptr; P.colidx = a->colidx; P.a = a->a; P.x = a->x; P.y = a->y; P.b = a->b;
-        P.acc = a->acc; P.dotrows = a->dotrows; P.mode = a->mode;
-        P.ctrl_in = a->ctrl_in; P.ctrl_out = a->ctrl_out; P.st = a->st; P.housekeeping = a->housekeeping;
-        P.p2p = (acgb200_p2pdev *) a->p2p; P.od_rowoffset = a->od_rowoffset; P.od_nrows = a->od_nrows;
-        P.orowptr = a->orowptr; P.ocolidx = a->ocolidx; P.oa = a->oa; P.pub_ch = a->p2p ? a->pub_ch : -1;
-        const cudaError_t le = launch_chain(spmv_variant(pl->lanes_per_row, pl->threads, pl->unroll),
-                                            pl->grid, pl->threads, (size_t) pl->smem_bytes, stream, P);
-        if (le) return (int) le;
-        cudaError_t err = cudaGetLastError();
-        if (err) return (int) err;
+        const int err = launch_tiles(a, stream);
+        if (err) return err;
     }
     if (pl->nmed > 0) {
         long long grid = ((long long) pl->nmed + 7) / 8;
@@ -2327,6 +2468,47 @@ extern "C" int acgb200_pcg_update(int n, acgb200_devstate *st, int cin, int cout
     static int occ = 0;
     return (int) launch_chain(pcg_update_kernel, blas1_grid(n, (const void *) pcg_update_kernel, &occ), BLAS1_THREADS, 0, stream,
                               n, st, cin, cout, multi, p2p, q, z, w, t, p, r, x);
+}
+
+extern "C" int acgb200_pcg_fused_launch(const acgb200_pcgargs *a, cudaStream_t stream)
+{
+    const acgb200_spmvplan *pl = a->plan;
+    if (pl->symdiag_nd <= 0 || pl->pcg_grid <= 0 || pl->nmtiles > 0 || pl->nmed > 0 || pl->nlong > 0)
+        return (int) cudaErrorInvalidConfiguration;
+    acgb200_ctrl *ctrl = a->st->ctrl;
+    const int cout = a->cin ^ 1;
+    int fin = a->cin;                   /* the control word the fused kernel reads */
+    if (pl->ntiles > 0) {
+        /* rows outside the slices: q = A w over the tiles, then their update (control words cin -> 2 -> 3) */
+        acgb200_spmvargs s;
+        memset(&s, 0, sizeof(s));
+        s.plan = pl; s.rowptr = a->rowptr; s.colidx = a->colidx; s.a = a->a; s.x = a->w; s.y = a->q;
+        s.mode = SPMV_Y_AX; s.ctrl_in = &ctrl[a->cin]; s.ctrl_out = &ctrl[2]; s.st = a->st;
+        int err = launch_tiles(&s, stream);
+        if (err) return err;
+        long long grid = pl->ntiles;
+        const long long cap = (long long) acgb200_num_sms() * 8;
+        if (grid > cap) grid = cap;
+        const cudaError_t le = launch_chain(pcg_tail_update_kernel, (int) grid, PCG_TAIL_THREADS, 0, stream,
+                                            (const acgb200_tile *) pl->d_tiles, pl->ntiles, a->st,
+                                            (const acgb200_ctrl *) &ctrl[2], &ctrl[3], (const double *) a->q, a->w,
+                                            a->w_next, a->z, a->t, a->p, a->r, a->x);
+        if (le) return (int) le;
+        fin = 3;
+    }
+    SymdiagParams S;
+    memset(&S, 0, sizeof(S));
+    S.slices = pl->d_slices; S.nslices = pl->nslices; S.no = pl->symdiag_no; S.nrows = pl->nrows;
+    S.evict_first = pl->symdiag_evict_first; S.hval = pl->d_hval;
+    memcpy(S.tab, pl->symdiag_tab, sizeof(S.tab));
+    S.x = a->w; S.mode = SPMV_Y_AX;
+    S.ctrl_in = &ctrl[fin]; S.ctrl_out = &ctrl[cout]; S.st = a->st;
+    S.z = a->z; S.t = a->t; S.p = a->p; S.r = a->r; S.xs = a->x; S.w_next = a->w_next;
+    S.vec_evict_first = a->vec_evict_first;
+    const cudaError_t le = launch_chain(symdiag_variant(pl->slice_ub, pl->slice_threads, true), pl->pcg_grid, pl->slice_threads,
+                                        (size_t) 0, stream, S);
+    if (le) return (int) le;
+    return (int) cudaGetLastError();
 }
 
 extern "C" int acgb200_comm_post(const acgb200_postargs *a, cudaStream_t stream)

@@ -19,6 +19,19 @@ int64_t acgb200_spmv_min_bytes(const struct acgb200_spmvplan *pl)
            + pl->slice_excnnz * 4 + pl->slice_exc * 8;
 }
 
+/* fused pipelined CG, per covered row: the stored diagonals, w_i, reads of z t p r x, writes of z t p x r w' */
+int64_t acgb200_pcg_fused_min_bytes(const struct acgb200_spmvplan *pl)
+{
+    return (int64_t) pl->slice_rows * (8 * pl->symdiag_nd + 96);
+}
+
+/* the whole fused iteration: the tile kernel's product, the tile rows' update (7 reads, 6 writes), the fused launch */
+int64_t acgb200_pcg_iteration_min_bytes(const struct acgb200_spmvplan *pl)
+{
+    const int64_t tnnz = pl->nnz - pl->slice_nnz, trows = pl->nrows - pl->slice_rows;
+    return tnnz * 12 + trows * (20 + 104) + acgb200_pcg_fused_min_bytes(pl);
+}
+
 /*
  * Tile-plan heuristic, from sweeps of tile shapes (tools/sweep.py).  The
  * compute phase of a tile is a chain LDS(col) -> LDG(x) -> DFMA per nonzero and

@@ -22,7 +22,9 @@ extern "C" {
  * of an exactly symmetric matrix read each stored value once -- the upper diagonals, every lower entry from its
  * mirror row -- when the structure allows, slices.c; "symdiag_evict_first" 0/1 their L2 policy), "spmv_merge" (-1/0/1,
  * default -1: merge-path tiles when the row lengths are irregular, mergeplan.c; "merge_items", "merge_threads",
- * "merge_max_ctas"), "spmv_medium", "graph"
+ * "merge_max_ctas"), "pcg_fused" (1/0, default 1: pipelined CG on one GPU runs each iteration's product and
+ * vector update in one kernel when the plan has mirrored diagonals and no merge tiles, medium or long rows;
+ * "pcg_evict_first" 1/0 the L2 policy of its vector streams), "spmv_medium", "graph"
  * (0/1: replay iteration pairs as CUDA graphs), "redstream" (0/1: pipelined
  * allreduce on its own stream and communicator; read at acgsolvercuda_init).  Environment variables ACGB200_<KEY> set the
  * same values at first use. */
@@ -133,6 +135,10 @@ struct acgb200_info {
     int spmv_symdiag_diagonals;                 /* upper diagonals stored for the slice-covered rows, whose lower entries
                                                    come from their mirror rows (option "spmv_symdiag"); 0: off */
     int64_t spmv_symdiag_bytes;                 /* their bytes, zero margins included */
+    int pcg_fused;                              /* 1: the last solve was pipelined CG with each iteration's product
+                                                   and update fused (option "pcg_fused"); spmv_min_bytes and
+                                                   last_spmv_ms then cover the whole iteration, last_blas_ms is 0 */
+    int64_t pcg_fused_min_bytes;                /* bytes the fused kernel moves at least: 8 |D| + 96 per slice row */
 };
 ACG_API int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info);
 
