@@ -129,7 +129,8 @@ class acgb200_info(C.Structure):
                                 "spmv_merge_grid", "spmv_merge_stages")] + \
         [("spmv_slice_value_bytes", C.c_int64), ("spmv_slice_nnz", C.c_int64)] + \
         [("spmv_symdiag_diagonals", C.c_int), ("spmv_symdiag_bytes", C.c_int64)] + \
-        [("pcg_fused", C.c_int), ("pcg_fused_min_bytes", C.c_int64)]
+        [("pcg_fused", C.c_int), ("pcg_fused_min_bytes", C.c_int64)] + \
+        [("spmv_symdiag_codes", C.c_int), ("spmv_symdiag_code_bytes", C.c_int64)]
 
 
 class acgb200_colstats(C.Structure):

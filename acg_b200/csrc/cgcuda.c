@@ -62,12 +62,14 @@ static struct {
     int slice_ub, slice_threads, slice_max_ctas;   /* slice kernel shape overrides (0 = default) */
     int spmv_symdiag;   /* 1: mirrored diagonals for the slice-covered rows when the matrix allows (slices.c), 0: off */
     int symdiag_evict_first;   /* 1: L2 evict-first policy on the stored diagonals (A/B; the default reuses them in L2) */
+    int symdiag_codes;  /* 1: store the diagonals as one-byte codes into a table when they hold at most 256 distinct
+                         * values (automatic), 0: always the fp64 diagonals (A/B) */
     int pcg_fused;      /* 1: pipelined CG runs each iteration's product and update in one kernel where the plan allows
                          * (one GPU, mirrored diagonals; DESIGN.md section 4a), 0: off (A/B) */
     int pcg_evict_first;   /* 1: L2 evict-first policy on the fused kernel's vector streams (A/B) */
     int loaded;
 } cfg = { .check_every = 8, .graph = 1, .redstream = 1, .p2p = 1, .p2p_fuse = 1, .spmv_slices = 1, .spmv_merge = -1,
-          .spmv_symdiag = 1, .pcg_fused = 1, .pcg_evict_first = 1 };
+          .spmv_symdiag = 1, .symdiag_codes = 1, .pcg_fused = 1, .pcg_evict_first = 1 };
 
 static void cfg_load(void)
 {
@@ -102,6 +104,7 @@ static void cfg_load(void)
     if ((s = getenv("ACGB200_SLICE_MAX_CTAS"))) cfg.slice_max_ctas = atoi(s);
     if ((s = getenv("ACGB200_SPMV_SYMDIAG"))) cfg.spmv_symdiag = atoi(s);
     if ((s = getenv("ACGB200_SYMDIAG_EVICT_FIRST"))) cfg.symdiag_evict_first = atoi(s);
+    if ((s = getenv("ACGB200_SYMDIAG_CODES"))) cfg.symdiag_codes = atoi(s);
     if ((s = getenv("ACGB200_PCG_FUSED"))) cfg.pcg_fused = atoi(s);
     if ((s = getenv("ACGB200_PCG_EVICT_FIRST"))) cfg.pcg_evict_first = atoi(s);
     acgb200_blas1_set_ctas_per_sm(cfg.blas1_ctas);
@@ -138,6 +141,7 @@ int acgb200_set_option(const char *key, int value)
     else if (!strcmp(key, "slice_max_ctas")) cfg.slice_max_ctas = value;
     else if (!strcmp(key, "spmv_symdiag")) cfg.spmv_symdiag = value;
     else if (!strcmp(key, "symdiag_evict_first")) cfg.symdiag_evict_first = value;
+    else if (!strcmp(key, "symdiag_codes")) cfg.symdiag_codes = value;
     else if (!strcmp(key, "pcg_fused")) cfg.pcg_fused = value;
     else if (!strcmp(key, "pcg_evict_first")) cfg.pcg_evict_first = value;
     else return ACG_ERR_INVALID_VALUE;
@@ -281,7 +285,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
         for (int i = 0; i < 4; i++) if (pv->graph[i]) cudaGraphExecDestroy(pv->graph[i]);
         cudaFree(pv->plan.d_tiles); cudaFree(pv->plan.d_longrows); cudaFree(pv->plan.d_long_scratch); cudaFree(pv->plan.d_medrows);
         cudaFree(pv->plan.d_slices); cudaFree(pv->plan.d_sval); cudaFree(pv->plan.d_spatoff); cudaFree(pv->plan.d_spatid);
-        cudaFree(pv->plan.d_hval); cudaFree(pv->plan.d_symdiag_bad);
+        cudaFree(pv->plan.d_hval); cudaFree(pv->plan.d_symdiag_bad); cudaFree(pv->plan.d_hcode); cudaFree(pv->plan.d_codes);
         cudaFree(pv->plan.d_mtiles); cudaFree(pv->plan.d_msplit); cudaFree(pv->plan.d_mpart);
         cudaFree(pv->d_st);
         cudaFreeHost(pv->h_ctrl); cudaFreeHost(pv->h_st);
@@ -809,6 +813,9 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
                 if (!e) e = cudaMalloc((void **) &pl->d_symdiag_bad, sizeof(int));
                 /* "failed" until the device check has run and passed */
                 if (!e) { const int one = 1; e = cudaMemcpy(pl->d_symdiag_bad, &one, sizeof(int), cudaMemcpyHostToDevice); }
+                /* room for the coded layout, which the fill builds and checks too */
+                if (!e && cfg.symdiag_codes) e = cudaMalloc((void **) &pl->d_hcode, (size_t) sd.nd * (size_t) pl->symdiag_stride);
+                if (!e && cfg.symdiag_codes) e = cudaMalloc((void **) &pl->d_codes, sizeof(struct acgb200_codestate));
                 if (e) { *errcode = (int) e; err = ACG_ERR_CUDA; }
             }
         }
@@ -830,6 +837,22 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
             CU(cudaMemcpy(&bad, pl->d_symdiag_bad, sizeof(int), cudaMemcpyDeviceToHost));
             CU(cudaFree(pl->d_symdiag_bad));
             pl->d_symdiag_bad = NULL;
+            int ncodes = 0;
+            if (!bad && pl->d_codes) {
+                /* the codes reproduce every stored double bit for bit: they replace the fp64 diagonals */
+                int st[2] = { 0, 1 };
+                CU(cudaMemcpy(st, (const char *) pl->d_codes + offsetof(struct acgb200_codestate, ncodes), sizeof(st),
+                              cudaMemcpyDeviceToHost));
+                if (st[0] >= 1 && st[0] <= ACGB200_CODES_MAX && !st[1]) ncodes = st[0];
+            }
+            if (bad || !ncodes) {
+                /* more than 256 values, or no codes asked for: the fp64 diagonals */
+                CU(cudaFree(pl->d_hcode)); CU(cudaFree(pl->d_codes));
+                pl->d_hcode = NULL; pl->d_codes = NULL;
+            } else {
+                CU(cudaFree(pl->d_hval));
+                pl->d_hval = NULL; pl->symdiag_codes = ncodes;
+            }
             if (bad) {
                 /* not exactly symmetric (or the check did not run): the slice kernel reads both triangles */
                 CU(cudaFree(pl->d_hval));
@@ -2434,5 +2457,7 @@ int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info
     info->spmv_symdiag_bytes = (int64_t) pv->plan.symdiag_nd * pv->plan.symdiag_stride * (int64_t) sizeof(double);
     info->pcg_fused = pv->last_fused;
     info->pcg_fused_min_bytes = pv->plan.symdiag_nd > 0 ? acgb200_pcg_fused_min_bytes(&pv->plan) : 0;
+    info->spmv_symdiag_codes = pv->plan.symdiag_codes;
+    info->spmv_symdiag_code_bytes = pv->plan.symdiag_codes > 0 ? (int64_t) pv->plan.symdiag_nd * pv->plan.symdiag_stride : 0;
     return ACG_SUCCESS;
 }

@@ -86,9 +86,15 @@ struct acgb200_spmvplan {
     int symdiag_d[ACGB200_SYMDIAG_MAX];   /* the stored diagonals D, ascending */
     int symdiag_margin;              /* zero entries in front of each diagonal (>= max D) */
     int symdiag_evict_first;         /* 1: stream the stored values with an L2 evict-first policy */
-    double *d_hval;                  /* [symdiag_nd * symdiag_stride] */
+    double *d_hval;                  /* [symdiag_nd * symdiag_stride]; NULL once the coded layout replaced it */
     const int *symdiag_colidx;       /* device CSR columns the fill reads (borrowed, valid during init only) */
     int *d_symdiag_bad;              /* fill-time symmetry check: 0 passed (written by acgb200_slices_fill) */
+    /* coded layout: when the stored diagonals hold at most 256 distinct bit patterns, one byte per element in
+     * the same layout (d_hcode[voff + i] in place of d_hval[voff + i]) indexes a table of those doubles,
+     * sorted by bit pattern.  Built and checked by acgb200_slices_fill when d_hcode and d_codes are set. */
+    int symdiag_codes;               /* table entries; 0: the fp64 diagonals */
+    uint8_t *d_hcode;                /* [symdiag_nd * symdiag_stride] */
+    struct acgb200_codestate *d_codes;   /* the table and the state of building it */
     int pcg_grid;                    /* grid of the fused pipelined-CG kernel (acgb200_pcg_fused_launch); 0: none */
     /* merge-path tiles (mergeplan.c): rows [0, merge_rows) of an irregular (power-law) matrix, cut into tiles
      * of merge_items merged items (row ends + nonzeros) and multiplied by spmv_merge_kernel; rows cut by tile
@@ -155,8 +161,23 @@ int acgb200_symdiag_plan(int nrows, const struct acgb200_sliceplan *sp, const st
 void acgb200_symdiag_layout(int nrows, const struct acgb200_symdiag *sd, int *margin, int *stride,
                             struct acgb200_symdiag_entry *tab);
 
+/* Building the coded layout (kernels.cu): the distinct bit patterns of the stored diagonals go into an
+ * open-addressing set, are sorted into vtab and every element is encoded, then decoded again and compared.
+ * The host reads ncodes and bad once the fill has finished: 1 <= ncodes <= 256 and bad == 0 mean the codes
+ * reproduce every stored double bit for bit. */
+#define ACGB200_CODES_MAX 256
+#define ACGB200_CODES_SET 1024       /* slots of the set; more than 256 patterns is an overflow before it fills */
+struct acgb200_codestate {
+    double vtab[ACGB200_CODES_MAX];  /* code c stands for vtab[c]; ascending by bit pattern */
+    unsigned long long set[ACGB200_CODES_SET];   /* distinct patterns; all ones marks an empty slot ... */
+    int has_ones;                    /* ... so that pattern itself (a NaN) is recorded here */
+    int overflow;                    /* more than 256 distinct patterns */
+    int ncodes;                      /* table entries; 0: no codes */
+    int bad;                         /* 1: an element was not reproduced by its code */
+};
+
 /* fill d_sval from the device CSR values (kernels.cu); with pl->d_hval also the mirrored diagonals and
- * their symmetry check (pl->d_symdiag_bad) */
+ * their symmetry check (pl->d_symdiag_bad), and with pl->d_hcode their codes (pl->d_codes) */
 int acgb200_slices_fill(const struct acgb200_spmvplan *pl, const int *d_rowptr, const double *d_a, cudaStream_t stream);
 
 /* row-pattern dictionary (compress.c): rows whose pattern id is not

@@ -28,6 +28,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
+#include <type_traits>
 
 #define SPMV_THREADS 128
 /* Resident CTAs per SM the register allocator must leave room for.  Without
@@ -118,6 +119,14 @@ __device__ __forceinline__ double ld_stream(const double *p, uint64_t pol)
 {
     double v;
     asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(v) : "l"(p), "l"(pol));
+    return v;
+}
+
+/* the same for one-byte value codes (the coded mirrored diagonals), zero-extended into a register */
+__device__ __forceinline__ unsigned ld_stream(const uint8_t *p, uint64_t pol)
+{
+    unsigned v;
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u8 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
     return v;
 }
 
@@ -770,7 +779,10 @@ struct SymdiagParams {
     int no;                        /* entries per row, |O| */
     int nrows;                     /* columns are clamped to [0, nrows) */
     int evict_first;
-    const double *hval;            /* the stored diagonals */
+    const double *hval;            /* the stored diagonals (fp64 layout) */
+    const uint8_t *hcode;          /* ... or one code per element, in the same layout (coded layout) */
+    const double *vtab;            /* the codes' values, ncodes <= 256 of them */
+    int ncodes;
     acgb200_symdiag_entry tab[ACGB200_SYMDIAG_MAX];   /* (value offset, column offset) per entry, O ascending */
     const double *x;
     double *y;
@@ -804,12 +816,22 @@ struct SymdiagParams {
  * and goes straight into the update (pcg_row) instead of to memory; the kernel is the iteration's last, so
  * block 0 advances the control word and zeroes ring slot (k+2) % 3 while every CTA adds into (k+1) % 3.
  * A met convergence test returns before the product.  At most 40 registers: 12 CTAs of 128 threads.
+ *
+ * V: double reads the fp64 diagonals (hval); uint8_t reads one code per element (hcode) and decodes it from
+ * a copy of the value table in shared memory just before the FMAs -- the same double, bit for bit, so the
+ * same sums.  The codes of a batch are loaded with the values' L2 policy, 32 bytes per warp and entry.
  */
-template <int UB, int T, bool PCG>
+__device__ __forceinline__ double sd_decode(double v, const double *) { return v; }
+__device__ __forceinline__ double sd_decode(unsigned c, const double *vtab_s) { return vtab_s[c]; }
+
+template <int UB, int T, bool PCG, typename V>
 __global__ void __launch_bounds__(T, PCG ? 1536 / T : 0)
 spmv_symdiag_kernel(const SymdiagParams P)
 {
+    constexpr bool CODED = std::is_same<V, uint8_t>::value;
+    typedef decltype(ld_stream((const V *) nullptr, 0)) R;      /* a loaded value or code */
     __shared__ int2 tab_s[ACGB200_SYMDIAG_MAX];
+    __shared__ double vtab_s[CODED ? 256 : 1];
     __shared__ double red[T / 32];
     const int tid = threadIdx.x;
     pdl_prologue();
@@ -838,6 +860,7 @@ spmv_symdiag_kernel(const SymdiagParams P)
     }
     if (!gate.active) return;
     if (tid < P.no) tab_s[tid] = make_int2(P.tab[tid].voff, P.tab[tid].coff);
+    if (CODED) for (int i = tid; i < P.ncodes; i += T) vtab_s[i] = __ldg(P.vtab + i);
     __syncthreads();
 
     /* L2 policy of the values: see the measurements in DESIGN section 3a */
@@ -852,24 +875,30 @@ spmv_symdiag_kernel(const SymdiagParams P)
     const uint64_t vpol = PCG ? (P.vec_evict_first ? l2_policy_evict_first() : l2_policy_evict_normal()) : 0;
     for (int s = warp; s < P.nslices; s += nwarps) {
         const int row = __ldg(&P.slices[s].row0) + lane;
-        const double *hv = P.hval + row;
+        const V *hv = (CODED ? (const V *) P.hcode : (const V *) P.hval) + row;
         double sum = 0.0;
         int e = 0;
         for (; e + UB <= L; e += UB) {
+            R cv[UB];
             double vv[UB], xv[UB];
 #pragma unroll
-            for (int u = 0; u < UB; u++) vv[u] = ld_stream(hv + tab_s[e + u].x, pol);
+            for (int u = 0; u < UB; u++) cv[u] = ld_stream(hv + tab_s[e + u].x, pol);
 #pragma unroll
             for (int u = 0; u < UB; u++) xv[u] = ld_x(P.x + min(max(row + tab_s[e + u].y, 0), cmax));
+#pragma unroll
+            for (int u = 0; u < UB; u++) vv[u] = sd_decode(cv[u], vtab_s);
             sum = slice_fma<UB>(vv, xv, sum);
         }
         if (e < L) {
             /* last, partial batch: slots past L are neither loaded nor added */
+            R cv[UB];
             double vv[UB], xv[UB];
 #pragma unroll
-            for (int u = 0; u < UB; u++) vv[u] = e + u < L ? ld_stream(hv + tab_s[e + u].x, pol) : 0.0;
+            for (int u = 0; u < UB; u++) cv[u] = e + u < L ? ld_stream(hv + tab_s[e + u].x, pol) : (R) 0;
 #pragma unroll
             for (int u = 0; u < UB; u++) xv[u] = e + u < L ? ld_x(P.x + min(max(row + tab_s[e + u].y, 0), cmax)) : 0.0;
+#pragma unroll
+            for (int u = 0; u < UB; u++) vv[u] = sd_decode(cv[u], vtab_s);
 #pragma unroll
             for (int u = 0; u < UB; u++) if (e + u < L) sum = fma(vv[u], xv[u], sum);
         }
@@ -889,7 +918,9 @@ spmv_symdiag_kernel(const SymdiagParams P)
         dot = block_sum(dot, red);
         dot2 = block_sum(dot2, red);
         if (tid == 0) {
-            double *acc = P.st->gd_loc[(gate.iter + 1) % 3];
+            /* coded: the iteration index read again rather than kept live through the loop (the word this
+             * kernel reads is not written during it) -- the UB = 9 loop would otherwise spill it */
+            double *acc = P.st->gd_loc[((CODED ? P.ctrl_in->iter : gate.iter) + 1) % 3];
             atomicAdd(&acc[0], dot);
             atomicAdd(&acc[1], dot2);
         }
@@ -941,6 +972,129 @@ symdiag_check_kernel(SymdiagParams P, const int *__restrict__ rowptr, const int 
             if (__double_as_longlong(want) != __double_as_longlong(got)) *bad = 1;
         }
     }
+}
+
+/* ---- the coded layout (once, at init): distinct bit patterns -> sorted table -> codes -> check ---- */
+
+#define CODES_EMPTY 0xFFFFFFFFFFFFFFFFull
+
+__device__ __forceinline__ unsigned codes_hash(unsigned long long v)
+{
+    return (unsigned) ((v * 0x9E3779B97F4A7C15ull) >> 54) & (ACGB200_CODES_SET - 1);
+}
+
+/* insert v (not CODES_EMPTY) into an open-addressing set of ACGB200_CODES_SET slots; 1: newly inserted,
+ * 0: already there, -1: the set is full */
+__device__ __forceinline__ int codes_insert(unsigned long long *set, unsigned long long v)
+{
+    unsigned h = codes_hash(v);
+    for (int probe = 0; probe < ACGB200_CODES_SET; probe++) {
+        const unsigned long long old = atomicCAS(set + h, CODES_EMPTY, v);
+        if (old == CODES_EMPTY) return 1;
+        if (old == v) return 0;
+        h = (h + 1) & (ACGB200_CODES_SET - 1);
+    }
+    return -1;
+}
+
+/* The distinct bit patterns of the n stored elements into cs->set.  Each CTA dedupes into a set in shared
+ * memory first (and each thread skips a repeat of its previous element), so the ~10^8 elements of a
+ * stencil matrix, nearly all one value, do not all contend for one global slot.  A CTA that sees more
+ * than 256 patterns sets cs->overflow and stops. */
+__global__ void __launch_bounds__(256)
+codes_collect_kernel(const unsigned long long *__restrict__ h, long long n, acgb200_codestate *cs)
+{
+    __shared__ unsigned long long set_s[ACGB200_CODES_SET];
+    __shared__ int n_s, ones_s;
+    for (int i = threadIdx.x; i < ACGB200_CODES_SET; i += blockDim.x) set_s[i] = CODES_EMPTY;
+    if (threadIdx.x == 0) { n_s = 0; ones_s = 0; }
+    __syncthreads();
+    unsigned long long last = CODES_EMPTY;
+    bool have = false;
+    for (long long i = blockIdx.x * (long long) blockDim.x + threadIdx.x; i < n; i += (long long) gridDim.x * blockDim.x) {
+        const unsigned long long v = __ldg(h + i);
+        if (have && v == last) continue;
+        last = v; have = true;
+        if (v == CODES_EMPTY) { ones_s = 1; continue; }
+        if (*(volatile int *) &n_s > ACGB200_CODES_MAX) break;
+        const int ins = codes_insert(set_s, v);
+        if (ins > 0) atomicAdd(&n_s, 1);
+        else if (ins < 0) { atomicAdd(&n_s, ACGB200_CODES_SET); break; }
+    }
+    __syncthreads();
+    if (n_s > ACGB200_CODES_MAX) { if (threadIdx.x == 0) cs->overflow = 1; return; }
+    if (threadIdx.x == 0 && ones_s) cs->has_ones = 1;
+    for (int i = threadIdx.x; i < ACGB200_CODES_SET; i += blockDim.x)
+        if (set_s[i] != CODES_EMPTY && codes_insert(cs->set, set_s[i]) < 0) cs->overflow = 1;
+}
+
+/* one CTA: the set's patterns sorted ascending by bit pattern into cs->vtab (the rank of each pattern is
+ * the number of smaller ones), cs->ncodes = their number, or 0 on overflow */
+__global__ void __launch_bounds__(1024)
+codes_sort_kernel(acgb200_codestate *cs)
+{
+    __shared__ unsigned long long k_s[ACGB200_CODES_SET + 1];
+    __shared__ int n_s;
+    if (threadIdx.x == 0) n_s = 0;
+    __syncthreads();
+    for (int i = threadIdx.x; i < ACGB200_CODES_SET; i += blockDim.x) {
+        const unsigned long long v = cs->set[i];
+        if (v != CODES_EMPTY) k_s[atomicAdd(&n_s, 1)] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && cs->has_ones) k_s[n_s++] = CODES_EMPTY;
+    __syncthreads();
+    const int n = n_s;
+    if (cs->overflow || n > ACGB200_CODES_MAX) { if (threadIdx.x == 0) cs->ncodes = 0; return; }
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const unsigned long long v = k_s[i];
+        int rank = 0;
+        for (int j = 0; j < n; j++) rank += k_s[j] < v;
+        cs->vtab[rank] = __longlong_as_double((long long) v);
+    }
+    if (threadIdx.x == 0) cs->ncodes = n;
+}
+
+/* code[i] = the index of h[i] in the sorted table (binary search; a thread reuses its previous element's
+ * code when the pattern repeats) */
+__global__ void __launch_bounds__(256)
+codes_encode_kernel(const unsigned long long *__restrict__ h, uint8_t *__restrict__ code, long long n,
+                    const acgb200_codestate *cs)
+{
+    __shared__ unsigned long long t_s[ACGB200_CODES_MAX];
+    const int nc = cs->ncodes;
+    if (nc == 0) return;
+    for (int i = threadIdx.x; i < nc; i += blockDim.x) t_s[i] = (unsigned long long) __double_as_longlong(cs->vtab[i]);
+    __syncthreads();
+    unsigned long long last = t_s[0];
+    int c = 0;
+    for (long long i = blockIdx.x * (long long) blockDim.x + threadIdx.x; i < n; i += (long long) gridDim.x * blockDim.x) {
+        const unsigned long long v = __ldg(h + i);
+        if (v != last) {
+            int lo = 0, hi = nc - 1;
+            while (lo < hi) { const int mid = (lo + hi) >> 1; if (t_s[mid] < v) lo = mid + 1; else hi = mid; }
+            last = v; c = lo;
+        }
+        code[i] = (uint8_t) c;
+    }
+}
+
+/* every code must decode to its element bit for bit; any difference sets cs->bad */
+__global__ void __launch_bounds__(256)
+codes_check_kernel(const unsigned long long *__restrict__ h, const uint8_t *__restrict__ code, long long n,
+                   acgb200_codestate *cs)
+{
+    __shared__ unsigned long long t_s[ACGB200_CODES_MAX];
+    const int nc = cs->ncodes;
+    if (nc == 0) return;
+    for (int i = threadIdx.x; i < nc; i += blockDim.x) t_s[i] = (unsigned long long) __double_as_longlong(cs->vtab[i]);
+    __syncthreads();
+    bool bad = false;
+    for (long long i = blockIdx.x * (long long) blockDim.x + threadIdx.x; i < n; i += (long long) gridDim.x * blockDim.x) {
+        const int c = code[i];
+        bad |= c >= nc || t_s[c] != __ldg(h + i);
+    }
+    if (__syncthreads_or(bad) && threadIdx.x == 0) cs->bad = 1;
 }
 
 /* ------------------------------------------------------------------------ */
@@ -2204,13 +2358,31 @@ static slice_fn slice_variant(int UB, int T, int EXC)
 typedef void (*symdiag_fn)(const SymdiagParams);
 
 /* the mirrored-diagonal kernel for exactly the (UB, T) pairs of slice_variant; pcg: with the fused
- * pipelined-CG epilogue */
-static symdiag_fn symdiag_variant(int UB, int T, bool pcg)
+ * pipelined-CG epilogue; coded: reading one-byte codes (the plan's symdiag_codes > 0) */
+static symdiag_fn symdiag_variant(int UB, int T, bool pcg, bool coded)
 {
-#define X(u, t) if (UB == u && T == t) return pcg ? spmv_symdiag_kernel<u, t, true> : spmv_symdiag_kernel<u, t, false>;
+#define X(u, t) if (UB == u && T == t) \
+        return coded ? (pcg ? spmv_symdiag_kernel<u, t, true, uint8_t> : spmv_symdiag_kernel<u, t, false, uint8_t>) \
+                     : (pcg ? spmv_symdiag_kernel<u, t, true, double> : spmv_symdiag_kernel<u, t, false, double>);
     X(5, 128) X(7, 128) X(8, 128) X(9, 128) X(7, 256) X(8, 256) X(9, 256)
 #undef X
     return NULL;
+}
+
+static symdiag_fn symdiag_variant(const acgb200_spmvplan *pl, bool pcg)
+{
+    return symdiag_variant(pl->slice_ub, pl->slice_threads, pcg, pl->symdiag_codes > 0);
+}
+
+/* the kernel's view of the plan's stored diagonals, fp64 or coded */
+static void symdiag_params(const acgb200_spmvplan *pl, SymdiagParams &S)
+{
+    S.slices = pl->d_slices; S.nslices = pl->nslices; S.no = pl->symdiag_no; S.nrows = pl->nrows;
+    S.evict_first = pl->symdiag_evict_first; S.hval = pl->d_hval;
+    S.hcode = pl->symdiag_codes > 0 ? pl->d_hcode : NULL;
+    S.vtab = pl->symdiag_codes > 0 ? pl->d_codes->vtab : NULL;
+    S.ncodes = pl->symdiag_codes;
+    memcpy(S.tab, pl->symdiag_tab, sizeof(S.tab));
 }
 
 typedef void (*merge_fn)(const MergeParams);
@@ -2261,7 +2433,7 @@ extern "C" int acgb200_spmv_configure(acgb200_spmvplan *pl)
     }
     if (pl->nslices > 0) {
         /* the mirrored-diagonal kernel, when the plan has them, takes the slice kernel's place and grid rule */
-        const void *sfn = pl->symdiag_nd > 0 ? (const void *) symdiag_variant(pl->slice_ub, pl->slice_threads, false)
+        const void *sfn = pl->symdiag_nd > 0 ? (const void *) symdiag_variant(pl, false)
                                              : (const void *) slice_variant(pl->slice_ub, pl->slice_threads, pl->slice_exc > 0);
         if (!sfn) return (int) cudaErrorInvalidConfiguration;
         pl->slice_smem = pl->symdiag_nd > 0 ? 0 : ((pl->slice_npat * pl->slice_lpad + 3) & ~3) * (int) sizeof(int);
@@ -2283,7 +2455,8 @@ extern "C" int acgb200_spmv_configure(acgb200_spmvplan *pl)
              * rule stands (DESIGN section 4a). */
             int dev = 0, l2 = 0;
             if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev) == cudaSuccess && l2 > 0) {
-                const long long row_bytes = 8LL * pl->symdiag_nd + 16;
+                /* one byte per diagonal in the coded layout: at C3 the cap (49) then no longer binds */
+                const long long row_bytes = (pl->symdiag_codes > 0 ? 1LL : 8LL) * pl->symdiag_nd + 16;
                 long long cap = (long long) l2 / 2 / ((long long) acgb200_num_sms() * pl->slice_threads * row_bytes);
                 if (cap < 1) cap = 1;
                 if (sper > cap) sper = (int) cap;
@@ -2297,7 +2470,7 @@ extern "C" int acgb200_spmv_configure(acgb200_spmvplan *pl)
         if (pl->symdiag_nd > 0) {
             /* the fused pipelined-CG kernel: the same grid, unless its registers allow fewer CTAs */
             int fper = 0;
-            err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fper, (const void *) symdiag_variant(pl->slice_ub, pl->slice_threads, true),
+            err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fper, (const void *) symdiag_variant(pl, true),
                                                                 pl->slice_threads, 0);
             if (err) return (int) err;
             const long long fgrid = (long long) acgb200_num_sms() * (fper < 1 ? 1 : fper);
@@ -2331,6 +2504,22 @@ extern "C" int acgb200_slices_fill(const acgb200_spmvplan *pl, const int *d_rowp
     symdiag_fill_kernel<<<(int) (fgrid < 1 ? 1 : fgrid), 256, 0, stream>>>(pl->nrows, d_rowptr, pl->symdiag_colidx, d_a, pl->d_hval,
                                                                           pl->symdiag_nd, D, pl->symdiag_stride, pl->symdiag_margin);
     symdiag_check_kernel<<<(int) grid, 256, 0, stream>>>(S, d_rowptr, pl->symdiag_colidx, d_a, pl->d_symdiag_bad);
+    err = cudaGetLastError();
+    if (err || !pl->d_hcode || !pl->d_codes) return (int) err;
+    /* the coded layout: distinct patterns, their sorted table, the codes and their check (each kernel after
+     * the sort finds ncodes == 0 on overflow and does nothing) */
+    acgb200_codestate *cs = pl->d_codes;
+    err = cudaMemsetAsync(cs, 0, sizeof(*cs), stream);
+    if (!err) err = cudaMemsetAsync(cs->set, 0xFF, sizeof(cs->set), stream);
+    if (err) return (int) err;
+    const long long n = (long long) pl->symdiag_nd * pl->symdiag_stride;
+    long long cgrid = (n + 255) / 256;
+    if (cgrid > cap) cgrid = cap;
+    const unsigned long long *h = (const unsigned long long *) pl->d_hval;
+    codes_collect_kernel<<<(int) cgrid, 256, 0, stream>>>(h, n, cs);
+    codes_sort_kernel<<<1, 1024, 0, stream>>>(cs);
+    codes_encode_kernel<<<(int) cgrid, 256, 0, stream>>>(h, pl->d_hcode, n, cs);
+    codes_check_kernel<<<(int) cgrid, 256, 0, stream>>>(h, pl->d_hcode, n, cs);
     return (int) cudaGetLastError();
 }
 
@@ -2382,12 +2571,10 @@ extern "C" int acgb200_spmv_launch(const acgb200_spmvargs *a, cudaStream_t strea
     }
     if (pl->nslices > 0 && pl->symdiag_nd > 0) {
         SymdiagParams S;
-        S.slices = pl->d_slices; S.nslices = pl->nslices; S.no = pl->symdiag_no; S.nrows = pl->nrows;
-        S.evict_first = pl->symdiag_evict_first; S.hval = pl->d_hval;
-        memcpy(S.tab, pl->symdiag_tab, sizeof(S.tab));
+        symdiag_params(pl, S);
         S.x = a->x; S.y = a->y; S.b = a->b; S.acc = a->acc; S.dotrows = a->dotrows; S.mode = a->mode;
         S.ctrl_in = a->ctrl_in; S.ctrl_out = slices_forward ? a->ctrl_out : NULL; S.st = a->st; S.housekeeping = a->housekeeping;
-        const cudaError_t le = launch_chain(symdiag_variant(pl->slice_ub, pl->slice_threads, false), pl->slice_grid, pl->slice_threads,
+        const cudaError_t le = launch_chain(symdiag_variant(pl, false), pl->slice_grid, pl->slice_threads,
                                             (size_t) 0, stream, S);
         if (le) return (int) le;
     } else if (pl->nslices > 0) {
@@ -2498,14 +2685,12 @@ extern "C" int acgb200_pcg_fused_launch(const acgb200_pcgargs *a, cudaStream_t s
     }
     SymdiagParams S;
     memset(&S, 0, sizeof(S));
-    S.slices = pl->d_slices; S.nslices = pl->nslices; S.no = pl->symdiag_no; S.nrows = pl->nrows;
-    S.evict_first = pl->symdiag_evict_first; S.hval = pl->d_hval;
-    memcpy(S.tab, pl->symdiag_tab, sizeof(S.tab));
+    symdiag_params(pl, S);
     S.x = a->w; S.mode = SPMV_Y_AX;
     S.ctrl_in = &ctrl[fin]; S.ctrl_out = &ctrl[cout]; S.st = a->st;
     S.z = a->z; S.t = a->t; S.p = a->p; S.r = a->r; S.xs = a->x; S.w_next = a->w_next;
     S.vec_evict_first = a->vec_evict_first;
-    const cudaError_t le = launch_chain(symdiag_variant(pl->slice_ub, pl->slice_threads, true), pl->pcg_grid, pl->slice_threads,
+    const cudaError_t le = launch_chain(symdiag_variant(pl, true), pl->pcg_grid, pl->slice_threads,
                                         (size_t) 0, stream, S);
     if (le) return (int) le;
     return (int) cudaGetLastError();

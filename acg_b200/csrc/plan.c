@@ -8,13 +8,17 @@
 
 #define SPMV_THREADS 128
 
+/* bytes per stored element of the mirrored diagonals: a double, or a one-byte code */
+static int64_t symdiag_elem_bytes(const struct acgb200_spmvplan *pl) { return pl->symdiag_codes > 0 ? 1 : 8; }
+
 int64_t acgb200_spmv_min_bytes(const struct acgb200_spmvplan *pl)
 {
     /* tiles: values + indices + per row: row pointer, y, x; slices: padded values + per row: pattern id, y, x */
     const int64_t tnnz = pl->nnz - pl->slice_nnz, trows = pl->nrows - pl->slice_rows;
-    /* mirrored diagonals: per covered row one value per stored diagonal (the lower entries come again from L2), y, x */
+    /* mirrored diagonals: per covered row one value (8 bytes, or a 1-byte code) per stored diagonal (the lower
+     * entries come again from L2), y, x */
     if (pl->symdiag_nd > 0)
-        return tnnz * 12 + trows * 20 + (int64_t) pl->slice_rows * (8 * pl->symdiag_nd + 16);
+        return tnnz * 12 + trows * 20 + (int64_t) pl->slice_rows * (symdiag_elem_bytes(pl) * pl->symdiag_nd + 16);
     return tnnz * 12 + trows * 20 + pl->sval_blocks * 256 + (int64_t) pl->slice_rows * 18
            + pl->slice_excnnz * 4 + pl->slice_exc * 8;
 }
@@ -22,7 +26,7 @@ int64_t acgb200_spmv_min_bytes(const struct acgb200_spmvplan *pl)
 /* fused pipelined CG, per covered row: the stored diagonals, w_i, reads of z t p r x, writes of z t p x r w' */
 int64_t acgb200_pcg_fused_min_bytes(const struct acgb200_spmvplan *pl)
 {
-    return (int64_t) pl->slice_rows * (8 * pl->symdiag_nd + 96);
+    return (int64_t) pl->slice_rows * (symdiag_elem_bytes(pl) * pl->symdiag_nd + 96);
 }
 
 /* the whole fused iteration: the tile kernel's product, the tile rows' update (7 reads, 6 writes), the fused launch */

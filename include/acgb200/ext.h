@@ -20,7 +20,8 @@ extern "C" {
  * (0/1, default 1: index-free slice-major storage of the rows that repeat a pattern, slices.c; shape
  * overrides "slice_ub", "slice_threads", "slice_max_ctas"), "spmv_symdiag" (1/0, default 1: the slice-covered rows
  * of an exactly symmetric matrix read each stored value once -- the upper diagonals, every lower entry from its
- * mirror row -- when the structure allows, slices.c; "symdiag_evict_first" 0/1 their L2 policy), "spmv_merge" (-1/0/1,
+ * mirror row -- when the structure allows, slices.c; "symdiag_evict_first" 0/1 their L2 policy; "symdiag_codes" 1/0,
+ * default 1: store them as one-byte codes into a table when they hold at most 256 distinct values), "spmv_merge" (-1/0/1,
  * default -1: merge-path tiles when the row lengths are irregular, mergeplan.c; "merge_items", "merge_threads",
  * "merge_max_ctas"), "pcg_fused" (1/0, default 1: pipelined CG on one GPU runs each iteration's product and
  * vector update in one kernel when the plan has mirrored diagonals and no merge tiles, medium or long rows;
@@ -134,11 +135,16 @@ struct acgb200_info {
     int64_t spmv_slice_nnz;                     /* nonzeros those slices cover (without padding) */
     int spmv_symdiag_diagonals;                 /* upper diagonals stored for the slice-covered rows, whose lower entries
                                                    come from their mirror rows (option "spmv_symdiag"); 0: off */
-    int64_t spmv_symdiag_bytes;                 /* their bytes, zero margins included */
+    int64_t spmv_symdiag_bytes;                 /* their bytes as doubles, zero margins included (with codes the
+                                                   device holds spmv_symdiag_code_bytes instead) */
     int pcg_fused;                              /* 1: the last solve was pipelined CG with each iteration's product
                                                    and update fused (option "pcg_fused"); spmv_min_bytes and
                                                    last_spmv_ms then cover the whole iteration, last_blas_ms is 0 */
-    int64_t pcg_fused_min_bytes;                /* bytes the fused kernel moves at least: 8 |D| + 96 per slice row */
+    int64_t pcg_fused_min_bytes;                /* bytes the fused kernel moves at least: 8 |D| + 96 per slice row
+                                                   (|D| + 96 with codes) */
+    int spmv_symdiag_codes;                     /* entries of the value table when the stored diagonals are one-byte
+                                                   codes into it (option "symdiag_codes"); 0: fp64 diagonals */
+    int64_t spmv_symdiag_code_bytes;            /* the codes' bytes, one per element of the diagonals; 0: no codes */
 };
 ACG_API int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info);
 
