@@ -162,7 +162,7 @@ EXPORTS = [
     "acgsolvercuda_init_constants", "acgsolvercuda_alpha", "acgsolvercuda_beta", "acgsolvercuda_daxpy_alpha",
     "acgsolvercuda_daxpy_minus_alpha", "acgsolvercuda_daypx_beta", "acgsolvercuda_pipelined_daxpy_fused",
     "acgsolvercuda_fwrite",
-    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_solve_multi", "acgsolvercuda_spmm_mode", "acgsolvercuda_solve_shifted", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
+    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_solve_multi", "acgsolvercuda_spmm_mode", "acgsolvercuda_solve_shifted", "acgsolvercuda_solve_minres", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
     "acgb200_nccl_unique_id", "acgb200_comm_init_rank", "acgb200_comm_destroy",
     "acgb200_host_register", "acgb200_host_unregister", "acgb200_spmv_plan_host", "acgb200_spmv_plan_host2", "acgb200_slices_host", "acgb200_symdiag_host", "acgb200_merge_plan_host", "acgb200_p2p_inverse_map", "acgb200_patterns_host", "acgb200_stencil_part",
     "acgb200_mtx_info", "acgb200_mtx_read", "acgb200_mtx_read_part", "acgb200_comm_matrix_row", "acgb200_partition_rows_grid", "acgb200_grid_factors", "acgb200_rmat_spd",
@@ -246,6 +246,8 @@ def lib() -> C.CDLL:
     L.acgsolvercuda_spmm_mode.argtypes = [P(acgsolvercuda), C.c_int, C.c_int, f64p, C.c_void_p, f64p, P(C.c_double)]
     L.acgsolvercuda_solve_shifted.argtypes = [P(acgsolvercuda), P(acgsymcsrmatrix), C.c_int, f64p, f64p, f64p, C.c_int,
                                               C.c_double, C.c_double, C.c_int, P(acgb200_colstats)]
+    L.acgsolvercuda_solve_minres.argtypes = [P(acgsolvercuda), P(acgsymcsrmatrix), P(acgvector), P(acgvector), C.c_int,
+                                             C.c_double, C.c_double, C.c_int, P(C.c_int)]
     L.acgsolvercuda_info.argtypes = [P(acgsolvercuda), P(acgb200_info)]
     L.acgb200_set_option.argtypes = [C.c_char_p, C.c_int]
     L.acgb200_nccl_unique_id.argtypes = [C.c_void_p]
@@ -786,6 +788,20 @@ class SolverCuda:
         if code != ACG_SUCCESS and (raise_on_not_converged or code != ACG_ERR_NOT_CONVERGED):
             raise AcgError(code, "acgsolvercuda_solve_shifted", 0)
         return code, X, [{n: getattr(s, n) for n, _ in acgb200_colstats._fields_} for s in st[:S]]
+
+    def solve_minres(self, b, x, maxits=100, residualatol=0.0, residualrtol=0.0, warmup=0,
+                     raise_on_not_converged=False):
+        """acgsolvercuda_solve_minres: MINRES on the solver's operator, which may be indefinite or singular
+        (one GPU, whole matrix).  b, x: Vectors as for ``solvempi``, x the initial guess, updated in place.
+        Stops by ``solvempi``'s rule on MINRES's recursively updated residual norm (``c.rnrm2``), or on an
+        exact Krylov breakdown.  Returns the code like ``solve()``."""
+        err = C.c_int(0)
+        code = lib().acgsolvercuda_solve_minres(C.byref(self.c), C.byref(self.A.c), C.byref(b.c), C.byref(x.c),
+                                                int(maxits), float(residualatol), float(residualrtol), int(warmup),
+                                                C.byref(err))
+        if code != ACG_SUCCESS and (raise_on_not_converged or code != ACG_ERR_NOT_CONVERGED):
+            raise AcgError(code, "acgsolvercuda_solve_minres", err.value)
+        return code
 
     def spmm_mode(self, mode: int, X: np.ndarray, B: np.ndarray | None = None):
         """The multi-vector product of solve_multi in one of the epilogue modes (acgsolvercuda_spmm_mode):

@@ -171,10 +171,10 @@ struct priv {
     struct acgcomm redcomm;             /* private duplicate of the caller's communicator for reductions */
     int have_redcomm;
     double *d_b, *d_x;                  /* right-hand side / solution on the device, kept between solves */
-    cudaGraphExec_t graph[4];           /* [0] classic, [1] pipelined, [2] several right-hand sides, [3] shifted
-                                         * systems: two iterations each (parity 0 then 1) */
-    int graph_sig[4];                   /* loop configuration each cached graph was captured with (graph_signature) */
-    int graph_launches[4];              /* kernel/NCCL launches inside one replay */
+    cudaGraphExec_t graph[5];           /* [0] classic, [1] pipelined, [2] several right-hand sides, [3] shifted
+                                         * systems, [4] MINRES: two iterations each (parity 0 then 1) */
+    int graph_sig[5];                   /* loop configuration each cached graph was captured with (graph_signature) */
+    int graph_launches[5];              /* kernel/NCCL launches inside one replay */
     double last_h2d_ms, last_d2h_ms;    /* host time spent before / after the solve window */
     cudaEvent_t ev_t0, ev_t1;           /* device-side bracket of the solve window */
     double last_solve_ms;
@@ -194,6 +194,10 @@ struct priv {
     int nranges, ranges_lanes, have_ranges;
     /* shifted systems (acgsolvercuda_solve_shifted): per-shift scalars; the vectors are the blocks above */
     struct acgb200_sstate *d_ss, *h_ss;
+    /* MINRES (acgsolvercuda_solve_minres), made at the first such solve: its scalars and the two w buffers
+     * (v lives in d_r / d_p, t and u in d_t) */
+    struct acgb200_nstate *d_ns, *h_ns;
+    double *d_nw[2];
 };
 
 /* The public struct has no room for private state (its layout is the
@@ -282,7 +286,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
             pv->p2p.window = NULL;
         }
         if (pv->have_redcomm && pv->redcomm.ncclcomm) ncclCommDestroy(pv->redcomm.ncclcomm);
-        for (int i = 0; i < 4; i++) if (pv->graph[i]) cudaGraphExecDestroy(pv->graph[i]);
+        for (int i = 0; i < 5; i++) if (pv->graph[i]) cudaGraphExecDestroy(pv->graph[i]);
         cudaFree(pv->plan.d_tiles); cudaFree(pv->plan.d_longrows); cudaFree(pv->plan.d_long_scratch); cudaFree(pv->plan.d_medrows);
         cudaFree(pv->plan.d_slices); cudaFree(pv->plan.d_sval); cudaFree(pv->plan.d_spatoff); cudaFree(pv->plan.d_spatid);
         cudaFree(pv->plan.d_hval); cudaFree(pv->plan.d_symdiag_bad); cudaFree(pv->plan.d_hcode); cudaFree(pv->plan.d_codes);
@@ -296,6 +300,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
         cudaFree(pv->d_b); cudaFree(pv->d_x); cudaFree(pv->d_w2);
         cudaFree(pv->d_ms); cudaFreeHost(pv->h_ms); cudaFree(pv->d_ranges);
         cudaFree(pv->d_ss); cudaFreeHost(pv->h_ss);
+        cudaFree(pv->d_ns); cudaFreeHost(pv->h_ns); cudaFree(pv->d_nw[0]); cudaFree(pv->d_nw[1]);
         cudaFree(pv->d_mx); cudaFree(pv->d_mb); cudaFree(pv->d_mr); cudaFree(pv->d_mp); cudaFree(pv->d_mt);
         if (pv->ev_ready) cudaEventDestroy(pv->ev_ready);
         if (pv->ev_halo) cudaEventDestroy(pv->ev_halo);
@@ -883,6 +888,7 @@ struct solvectx {
     int p2p;                  /* loop exchanges go through peer memory */
     int mk;                   /* multi-vector loop: block width K (0: single vector) */
     int shifted;              /* shifted-systems loop (acgsolvercuda_solve_shifted) */
+    int minres;               /* MINRES loop (acgsolvercuda_solve_minres) */
     int fused;                /* pipelined loop: one fused iteration (acgb200_pcg_fused_launch); its control word
                                * alternates between ctrl[0] and ctrl[1] by iteration parity */
     int issued;               /* iterations iterate() issued, inactive ones included */
@@ -1125,7 +1131,7 @@ static int graph_signature(const struct solvectx *c)
 {
     return 1 | (c->multi ? 2 : 0) | (c->p2p ? 4 : 0) | (c->pv->p2p.h_desc.fuse ? 8 : 0) | (cfg.pdl ? 16 : 0)
            | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0) | (c->shifted ? 128 : 0) | (c->mk << 8)
-           | (c->fused ? 1 << 16 : 0);
+           | (c->fused ? 1 << 16 : 0) | (c->minres ? 1 << 17 : 0);
 }
 
 static int capture_pair(struct solvectx *c, int kind, int (*issue)(struct solvectx *, int))
@@ -1866,6 +1872,199 @@ int acgsolvercuda_solve_shifted(struct acgsolvercuda *cg, const struct acgsymcsr
     pv->last_d2h_ms = 1e3 * (wall() - te);
     CU(cudaGetLastError());
     return status;
+}
+
+/* ------------------------------------------------------------------------ */
+/* MINRES: symmetric A that may be indefinite                                */
+/* ------------------------------------------------------------------------ */
+
+/* the MINRES kernels are linked in (see ACGB200_MULTI_LAUNCHER, internal.h) */
+static int have_minres_kernels(void)
+{
+    return acgb200_minres_setup && acgb200_minres_lanczos && acgb200_minres_update;
+}
+
+static int push_nstate(struct solvectx *c, const struct acgb200_nstate *ns)
+{
+    int *errcode = c->errcode;
+    CU(cudaStreamSynchronize(c->pv->stream));
+    *c->pv->h_ns = *ns;
+    CU(cudaMemcpyAsync(c->pv->d_ns, c->pv->h_ns, sizeof(*ns), cudaMemcpyHostToDevice, c->pv->stream));
+    CU(cudaStreamSynchronize(c->pv->stream));
+    return ACG_SUCCESS;
+}
+
+static int pull_nstate(struct solvectx *c, struct acgb200_nstate *ns)
+{
+    int *errcode = c->errcode;
+    CU(cudaMemcpyAsync(c->pv->h_ns, c->pv->d_ns, sizeof(*ns), cudaMemcpyDeviceToHost, c->pv->stream));
+    CU(cudaStreamSynchronize(c->pv->stream));
+    *ns = *c->pv->h_ns;
+    return ACG_SUCCESS;
+}
+
+/* r0 = b - A x into d_r with (r0,r0) folded in; *r0nrm2 = ||r0|| */
+static int minres_residual(struct solvectx *c, double *r0nrm2)
+{
+    struct priv *pv = c->pv;
+    struct acgb200_devstate h;
+    memset(&h, 0, sizeof(h));
+    OK(push_state(c, &h));
+    double rr = 0;
+    OK(apply_A(c, c->d_x, c->d_x, c->cg->d_r, c->d_b, SPMV_R_B_AX, &pv->d_st->tmp_loc[0], 0, 0, 0, -1));
+    OK(reduce_to_host(c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &rr));
+    *r0nrm2 = sqrt(rr);
+    return ACG_SUCCESS;
+}
+
+/* v_1 = r0 / beta_1 in d_r, v_0 = w_{-1} = w_0 = 0, and the scalars of the first iteration:
+ * beta_1, c_0 = -1, s_0 = 0, delta-bar_1 = epsilon_1 = 0, phi-bar_1 = beta_1 */
+static int minres_start(struct solvectx *c, int maxits, double tol, double beta1)
+{
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    KL(acgb200_minres_setup(pv->nowned, beta1 > 0 ? 1.0 / beta1 : 0.0, c->cg->d_r, c->cg->d_p, pv->d_nw[0], pv->d_nw[1],
+                            pv->stream));
+    c->launches += 1;
+    struct acgb200_nstate ns;
+    memset(&ns, 0, sizeof(ns));
+    ns.beta[0] = beta1; ns.cs[0] = -1.0; ns.phibar[0] = beta1;
+    OK(push_nstate(c, &ns));
+    struct acgb200_devstate h;
+    memset(&h, 0, sizeof(h));
+    h.maxits = maxits; h.tol = tol;
+    return push_state(c, &h);
+}
+
+/* iteration k: t = A v_k (+ alpha_k), u = t - alpha_k v_k - beta_k v_{k-1} (+ (u,u)), then the rotation, w_k, x
+ * and v_{k+1}.  v_k is in d_r for even k and in d_p for odd k, v_{k+1} goes over v_{k-1}, w_k over w_{k-2}. */
+static int minres_iteration(struct solvectx *c, int k)
+{
+    struct acgsolvercuda *cg = c->cg;
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    const int s = k & 1, n = pv->nowned;
+    double *v = s ? cg->d_p : cg->d_r, *vprev = s ? cg->d_r : cg->d_p;
+    OK(apply_A(c, v, v, cg->d_t, NULL, SPMV_Y_AX_DOT, &pv->d_ns->alpha[s], 1, 0, 0, 0));
+    prof_mark(c, &pv->blas);
+    KL(acgb200_minres_lanczos(n, pv->d_st, pv->d_ns, 1, v, vprev, cg->d_t, pv->stream));
+    KL(acgb200_minres_update(n, pv->d_st, pv->d_ns, 1, 0, v, cg->d_t, pv->d_nw[s], pv->d_nw[s ^ 1], c->d_x, vprev,
+                             pv->stream));
+    prof_mark(c, &pv->blas);
+    c->launches += 2;
+    return ACG_SUCCESS;
+}
+
+static void account_minres(struct acgsolvercuda *cg, const struct priv *pv, int nits)
+{
+    /* per iteration: the classic product with (v, Av) folded in; u = t - alpha v - beta v_prev with (u,u)
+     * (two axpys: t, v, v_prev read, u written) and w, x, v_{k+1} (three: v, u, both w, x read, w, x, v_{k+1}
+     * written) -- 96 bytes per row the two kernels move */
+    const int64_t n = pv->nowned, nnz = pv->fnnz + pv->onnz;
+    const int64_t bgemv = nnz * 12 + n * 16 + (int64_t) pv->nvec * 8;
+    cg->ngemv += nits; cg->nflops += (int64_t) nits * 3 * nnz; cg->Bgemv += (int64_t) nits * bgemv;
+    cg->ndot += nits; cg->nflops += (int64_t) nits * 2 * n; cg->Bdot += (int64_t) nits * 16 * n;
+    cg->nnrm2 += nits; cg->nflops += (int64_t) nits * 2 * n; cg->Bnrm2 += (int64_t) nits * 8 * n;
+    cg->naxpy += 5 * (int64_t) nits; cg->nflops += (int64_t) nits * 12 * n; cg->Baxpy += (int64_t) nits * 96 * n;
+}
+
+int acgsolvercuda_solve_minres(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A,
+                               const struct acgvector *b, struct acgvector *x, int maxits,
+                               double residualatol, double residualrtol, int warmup, int *errcode)
+{
+    int errcode_ = 0;
+    if (!errcode) errcode = &errcode_;
+    cfg_load();
+    struct priv *pv = priv_of(cg);
+    if (!pv || !A || !b || !x) return ACG_ERR_INVALID_VALUE;
+    if (!have_minres_kernels() || pv->nghost > 0 || pv->commsize > 1 || A->nghostrows > 0)
+        return ACG_ERR_NOT_SUPPORTED;      /* one GPU, whole matrix */
+    if (maxits < 0) return ACG_ERR_INVALID_VALUE;
+    struct acgcomm null;
+    memset(&null, 0, sizeof(null));
+    null.type = acgcomm_null;
+    struct solvectx c;
+    OK(solve_begin(&c, cg, A, b, x, 0.0, 0.0, &null, 0, errcode));
+    c.minres = 1;
+    const int n = pv->nowned;
+    if (!pv->d_ns) {
+        CU(cudaMalloc((void **) &pv->d_ns, sizeof(*pv->d_ns)));
+        CU(cudaMallocHost((void **) &pv->h_ns, sizeof(*pv->h_ns)));
+    }
+    for (int i = 0; i < 2; i++)
+        if (!pv->d_nw[i]) CU(cudaMalloc((void **) &pv->d_nw[i], ((size_t) pv->nvec + 2) * sizeof(double)));
+    struct acgb200_devstate h;
+    struct acgb200_nstate ns;
+
+    /* warm-up: the set-up and `warmup` iterations on x itself, then x0 again from the caller's vector */
+    if (warmup > 0) {
+        double beta1 = 0;
+        OK(minres_residual(&c, &beta1));
+        OK(minres_start(&c, warmup, 0.0, beta1));
+        for (int i = 0; i < warmup; i++) OK(minres_iteration(&c, i));
+        const double tb = wall();
+        const size_t nx = (size_t) (x->num_nonzeros < pv->nvec ? x->num_nonzeros : pv->nvec);
+        CU(cudaMemcpyAsync(c.d_x, x->x, nx * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
+        CU(cudaStreamSynchronize(pv->stream));
+        pv->last_h2d_ms += 1e3 * (wall() - tb);
+    }
+    if (cfg.profile) {
+        OK(evpool_reserve(&pv->gemv, 2 * (maxits + 2)));
+        OK(evpool_reserve(&pv->blas, 2 * (maxits + 2)));
+    }
+    pv->gemv.n = pv->blas.n = 0;
+
+    cg->nsolves++; cg->niterations = 0;
+    cg->bnrm2 = cg->r0nrm2 = cg->rnrm2 = cg->x0nrm2 = cg->dxnrm2 = INFINITY;
+    cg->maxits = maxits; cg->diffatol = 0; cg->diffrtol = 0;
+    cg->residualatol = residualatol; cg->residualrtol = residualrtol;
+    CU(cudaStreamSynchronize(pv->stream));
+    const double t0 = wall();
+    CU(cudaEventRecord(pv->ev_t0, pv->stream));
+    c.launches = 0;
+
+    /* ||b|| ; r0 = b - A x0 and beta_1 = ||r0|| */
+    memset(&h, 0, sizeof(h));
+    OK(push_state(&c, &h));
+    double bb = 0, beta1 = 0;
+    KL(acgb200_dot(n, c.d_b, c.d_b, &pv->d_st->tmp_loc[0], pv->stream));
+    OK(reduce_to_host(&c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &bb));
+    c.launches += 1;
+    cg->bnrm2 = sqrt(bb);
+    OK(minres_residual(&c, &beta1));
+    cg->rnrm2 = cg->r0nrm2 = beta1;
+    cg->nnrm2 += 2; cg->nflops += 4 * (int64_t) n; cg->Bnrm2 += 8 * (int64_t) n; cg->ngemv++;
+    const double tol = threshold(residualatol, residualrtol, beta1);
+    const double rtol_scaled = residualrtol * beta1;
+    int converged = tol > 0 && beta1 < tol;                        /* acg/cgcuda.c:836-842 */
+
+    /* beta_1 = 0: x0 solves the system, there is no Krylov space to build */
+    if (!converged && maxits > 0 && beta1 > 0) {
+        OK(minres_start(&c, maxits, tol, beta1));
+        OK(iterate(&c, maxits, tol > 0, 4, minres_iteration));
+        OK(pull_state(&c, &h));
+        OK(pull_nstate(&c, &ns));
+        cg->niterations = h.ctrl[0].iter;
+        cg->rnrm2 = ns.phibar[cg->niterations & 1];
+        converged = tol > 0 && cg->rnrm2 < tol;
+        cg->ntotaliterations += cg->niterations;
+    }
+    CU(cudaEventRecord(pv->ev_t1, pv->stream));
+    CU(cudaEventSynchronize(pv->ev_t1));
+    cg->tsolve += wall() - t0;
+    { float ms = 0; if (cudaEventElapsedTime(&ms, pv->ev_t0, pv->ev_t1) == cudaSuccess) pv->last_solve_ms = ms; }
+    account_minres(cg, pv, cg->niterations);
+    pv->last_launches = c.launches;
+    pv->last_fused = 0;
+    if (cfg.profile) {
+        pv->last_spmv_ms = evpool_sum_ms(&pv->gemv); pv->last_spmv_n = pv->gemv.n / 2;
+        pv->last_blas_ms = evpool_sum_ms(&pv->blas);
+        cg->tgemv += 1e-3 * pv->last_spmv_ms;
+        cg->taxpy += 1e-3 * pv->last_blas_ms;
+    }
+    int status = ACG_SUCCESS;
+    if (!converged && !(residualatol == 0 && rtol_scaled == 0)) status = ACG_ERR_NOT_CONVERGED;   /* :1099-1107 */
+    return solve_end(&c, x, status);
 }
 
 /* ------------------------------------------------------------------------ */

@@ -490,6 +490,40 @@ ACGB200_MULTI_LAUNCHER int acgb200_cg_shift_update(int n, int k, struct acgb200_
                                                    int cin, int cout, const double *r, double *p, double *x, double *pk,
                                                    cudaStream_t stream);
 
+/* ------------------------------------------------------------------------
+ * MINRES (acgsolvercuda_solve_minres): unpreconditioned Paige-Saunders on the
+ * single-vector product, for symmetric A that may be indefinite.  Iteration k
+ * (parity s = k&1) runs the product t = A v_k with alpha_k = (v_k, t) into
+ * alpha[s], the Lanczos kernel (u = t - alpha_k v_k - beta_k v_{k-1} in place
+ * in t, (u,u) into uu[s]) and the update kernel (Givens rotation, w_k, x,
+ * v_{k+1}).  v_{k+1} overwrites v_{k-1} and w_k overwrites w_{k-2}: two buffers
+ * each, chosen by parity.  The scalars of iteration k are read from slot s;
+ * block 0 of the update writes slot s^1 and zeroes alpha[s^1] and uu[s^1], so
+ * no kernel reads a slot it writes.
+ * ------------------------------------------------------------------------ */
+struct acgb200_nstate {
+    double alpha[2];                 /* (v_k, A v_k), accumulated by the product */
+    double uu[2];                    /* (u, u) = beta_{k+1}^2, accumulated by the Lanczos kernel */
+    double beta[2];                  /* beta_k */
+    double cs[2], sn[2];             /* the previous rotation c_{k-1}, s_{k-1} */
+    double dbar[2], eps[2];          /* delta-bar_k, epsilon_k */
+    double phibar[2];                /* phi-bar_k: the recursively updated residual norm */
+};
+/* set-up: v *= scale (v_1 = r_0 / beta_1), vprev = w0 = w1 = 0 */
+ACGB200_MULTI_LAUNCHER int acgb200_minres_setup(int n, double scale, double *v, double *vprev, double *w0, double *w1,
+                                                cudaStream_t stream);
+/* u = t - alpha_k v - beta_k vprev in place in t, (u,u) into ns->uu[k&1]; reads the control word ctrl[cin] */
+ACGB200_MULTI_LAUNCHER int acgb200_minres_lanczos(int n, const struct acgb200_devstate *st, struct acgb200_nstate *ns,
+                                                  int cin, const double *v, const double *vprev, double *t,
+                                                  cudaStream_t stream);
+/* The rotation from slot k&1 and beta_{k+1} = sqrt(uu), then w_k = (v - eps_k w_{k-2} - delta_k w_{k-1}) / gamma_k
+ * into w (which holds w_{k-2}), x += phi_k w_k, vnext = u / beta_{k+1}.  Block 0 writes slot (k&1)^1, ends the
+ * loop on phi-bar_{k+1} < tol or beta_{k+1} = 0 (after the update) or gamma_k = 0 (before it, the iteration not
+ * counted), zeroes the next accumulators and writes ctrl[cout]. */
+ACGB200_MULTI_LAUNCHER int acgb200_minres_update(int n, struct acgb200_devstate *st, struct acgb200_nstate *ns,
+                                                 int cin, int cout, const double *v, const double *u, double *w,
+                                                 const double *wprev, double *x, double *vnext, cudaStream_t stream);
+
 /* setup-time helpers */
 int acgb200_dot(int n, const double *x, const double *y, double *acc, cudaStream_t stream); /* acc += x.y */
 int acgb200_dot2(int n, const double *r, const double *w, double *acc2, cudaStream_t stream); /* acc2[0]+=r.r, acc2[1]+=w.r */

@@ -2252,6 +2252,135 @@ cg_shift_update_kernel(int n, acgb200_devstate *st, acgb200_sstate *ss, int cin,
     }
 }
 
+/* ---- MINRES -------------------------------------------------------------------------------------- */
+
+/* set-up of solve_minres: v_1 = r_0 / beta_1 in place (scale = 1 / beta_1), v_0 = w_{-1} = w_0 = 0 */
+__global__ void __launch_bounds__(BLAS1_THREADS)
+minres_setup_kernel(int n, double scale, double *__restrict__ v, double *__restrict__ vprev, double *__restrict__ w0,
+                    double *__restrict__ w1)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        v[i] = scale * v[i];
+        vprev[i] = 0.0; w0[i] = 0.0; w1[i] = 0.0;
+    }
+}
+
+/* u = t - alpha_k v_k - beta_k v_{k-1} in place in t (t = A v_k from the product, alpha_k its fused dot),
+ * and beta_{k+1}^2 = (u,u) in the same pass */
+__global__ void __launch_bounds__(BLAS1_THREADS)
+minres_lanczos_kernel(int n, const acgb200_devstate *st, acgb200_nstate *ns, int cin, const double *__restrict__ v,
+                      const double *__restrict__ vprev, double *__restrict__ t)
+{
+    __shared__ double red[BLAS1_THREADS / 32];
+    pdl_prologue();
+    const Gate g = gate_read(&st->ctrl[cin], st);
+    if (!g.active) return;
+    const int s = g.iter & 1;
+    const double al = ns->alpha[s], be = ns->beta[s];
+    double acc = 0.0;
+    const int n2 = n >> 1;
+    const double2 *v2 = reinterpret_cast<const double2 *>(v);
+    const double2 *q2 = reinterpret_cast<const double2 *>(vprev);
+    double2 *t2 = reinterpret_cast<double2 *>(t);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n2; i += gridDim.x * blockDim.x) {
+        const double2 vv = v2[i], qv = q2[i];
+        double2 tv = t2[i];
+        tv.x = fma(-be, qv.x, fma(-al, vv.x, tv.x));
+        tv.y = fma(-be, qv.y, fma(-al, vv.y, tv.y));
+        t2[i] = tv;
+        acc = fma(tv.x, tv.x, acc);
+        acc = fma(tv.y, tv.y, acc);
+    }
+    if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0) {
+        const double u = fma(-be, vprev[n - 1], fma(-al, v[n - 1], t[n - 1]));
+        t[n - 1] = u;
+        acc = fma(u, u, acc);
+    }
+    acc = block_sum(acc, red);
+    if (threadIdx.x == 0) atomicAdd(&ns->uu[s], acc);
+}
+
+/* The scalars of MINRES iteration k from slot s: the previous rotation applied to the new column of the
+ * Lanczos matrix, and the next rotation (scipy's minres, unpreconditioned).  gamma = 0 (only for singular
+ * A) leaves the rotation at zero: the update kernel stops before dividing by it. */
+struct MinresStep { double beta, delta, eps, gamma, cs, sn, phi, phibar, dbar, epsn; };
+
+__device__ __forceinline__ MinresStep minres_step(const acgb200_nstate *ns, int s)
+{
+    MinresStep o;
+    const double al = ns->alpha[s], cs = ns->cs[s], sn = ns->sn[s], dbar = ns->dbar[s], phibar = ns->phibar[s];
+    o.beta = sqrt(ns->uu[s]);
+    o.eps = ns->eps[s];
+    o.delta = cs * dbar + sn * al;
+    const double gbar = sn * dbar - cs * al;
+    o.epsn = sn * o.beta;
+    o.dbar = -cs * o.beta;
+    o.gamma = hypot(gbar, o.beta);
+    o.cs = o.gamma > 0.0 ? gbar / o.gamma : 0.0;
+    o.sn = o.gamma > 0.0 ? o.beta / o.gamma : 0.0;
+    o.phi = o.cs * phibar;
+    o.phibar = o.sn * phibar;
+    return o;
+}
+
+/* w_k = (v_k - eps_k w_{k-2} - delta_k w_{k-1}) / gamma_k into w (which held w_{k-2}), x += phi_k w_k,
+ * v_{k+1} = u / beta_{k+1} into vnext (which held v_{k-1}).  Every thread derives the scalars from slot s;
+ * block 0 writes slot s^1, applies the test phi-bar_{k+1} < tol, ends the loop on beta_{k+1} = 0 (exact
+ * breakdown: x is then the minimal-residual solution) or gamma_k = 0 (before the update, which is not
+ * counted), zeroes the next product's and Lanczos kernel's accumulators and advances the control word. */
+__global__ void __launch_bounds__(BLAS1_THREADS)
+minres_update_kernel(int n, acgb200_devstate *st, acgb200_nstate *ns, int cin, int cout, const double *__restrict__ v,
+                     const double *__restrict__ u, double *__restrict__ w, const double *__restrict__ wprev,
+                     double *__restrict__ x, double *__restrict__ vnext)
+{
+    pdl_prologue();
+    const Gate g = gate_read(&st->ctrl[cin], st);
+    const int s = g.iter & 1;
+    const MinresStep k = minres_step(ns, s);
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        acgb200_ctrl c = st->ctrl[cin];
+        if (g.active) {
+            if (k.gamma == 0.0) c.done = 1;
+            else {
+                c.iter = g.iter + 1;
+                ns->beta[s ^ 1] = k.beta; ns->cs[s ^ 1] = k.cs; ns->sn[s ^ 1] = k.sn;
+                ns->dbar[s ^ 1] = k.dbar; ns->eps[s ^ 1] = k.epsn; ns->phibar[s ^ 1] = k.phibar;
+                /* acg/cgcuda.c:1008-1012: the strict test, here on the recursively updated norm */
+                if (k.beta == 0.0 || (st->tol > 0.0 && k.phibar < st->tol)) c.done = 1;
+            }
+            ns->alpha[s ^ 1] = 0.0;        /* accumulators of the next product and Lanczos kernel */
+            ns->uu[s ^ 1] = 0.0;
+        }
+        st->ctrl[cout] = c;
+    }
+    if (!g.active || k.gamma == 0.0) return;
+    const double ig = 1.0 / k.gamma, ib = k.beta > 0.0 ? 1.0 / k.beta : 0.0;
+    const int n2 = n >> 1;
+    const double2 *v2 = reinterpret_cast<const double2 *>(v);
+    const double2 *u2 = reinterpret_cast<const double2 *>(u);
+    const double2 *p2 = reinterpret_cast<const double2 *>(wprev);
+    double2 *w2 = reinterpret_cast<double2 *>(w);
+    double2 *x2 = reinterpret_cast<double2 *>(x);
+    double2 *n2v = reinterpret_cast<double2 *>(vnext);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n2; i += gridDim.x * blockDim.x) {
+        const double2 vv = v2[i], uv = u2[i], pv = p2[i];
+        double2 wv = w2[i], xv = x2[i];
+        wv.x = fma(-k.delta, pv.x, fma(-k.eps, wv.x, vv.x)) * ig;
+        wv.y = fma(-k.delta, pv.y, fma(-k.eps, wv.y, vv.y)) * ig;
+        xv.x = fma(k.phi, wv.x, xv.x);
+        xv.y = fma(k.phi, wv.y, xv.y);
+        w2[i] = wv;
+        x2[i] = xv;
+        n2v[i] = make_double2(uv.x * ib, uv.y * ib);
+    }
+    if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0) {
+        const double wv = fma(-k.delta, wprev[n - 1], fma(-k.eps, w[n - 1], v[n - 1])) * ig;
+        w[n - 1] = wv;
+        x[n - 1] = fma(k.phi, wv, x[n - 1]);
+        vnext[n - 1] = u[n - 1] * ib;
+    }
+}
+
 /* ------------------------------------------------------------------------ */
 /* host-side launchers (C linkage)                                           */
 /* ------------------------------------------------------------------------ */
@@ -2853,6 +2982,32 @@ extern "C" int acgb200_cg_shift_update(int n, int k, acgb200_devstate *st, acgb2
                              BLAS1_THREADS, 0, stream, n, st, ss, cin, cout, r, p, x, pk)
     return (int) MULTI_K_DISPATCH(k, CALL);
 #undef CALL
+}
+
+extern "C" int acgb200_minres_setup(int n, double scale, double *v, double *vprev, double *w0, double *w1,
+                                    cudaStream_t stream)
+{
+    static int occ = 0;
+    minres_setup_kernel<<<blas1_grid(n, (const void *) minres_setup_kernel, &occ), BLAS1_THREADS, 0, stream>>>(
+        n, scale, v, vprev, w0, w1);
+    return (int) cudaGetLastError();
+}
+
+extern "C" int acgb200_minres_lanczos(int n, const acgb200_devstate *st, acgb200_nstate *ns, int cin, const double *v,
+                                      const double *vprev, double *t, cudaStream_t stream)
+{
+    static int occ = 0;
+    return (int) launch_chain(minres_lanczos_kernel, blas1_grid(n, (const void *) minres_lanczos_kernel, &occ),
+                              BLAS1_THREADS, 0, stream, n, st, ns, cin, v, vprev, t);
+}
+
+extern "C" int acgb200_minres_update(int n, acgb200_devstate *st, acgb200_nstate *ns, int cin, int cout, const double *v,
+                                     const double *u, double *w, const double *wprev, double *x, double *vnext,
+                                     cudaStream_t stream)
+{
+    static int occ = 0;
+    return (int) launch_chain(minres_update_kernel, blas1_grid(n, (const void *) minres_update_kernel, &occ),
+                              BLAS1_THREADS, 0, stream, n, st, ns, cin, cout, v, u, w, wprev, x, vnext);
 }
 
 extern "C" int acgb200_gather(int n, double *dst, const double *src, const int *idx, cudaStream_t stream)

@@ -105,6 +105,23 @@ ACG_API int acgsolvercuda_solve_shifted(struct acgsolvercuda *cg, const struct a
                                         int maxits, double residualatol, double residualrtol, int warmup,
                                         struct acgb200_colstats *stats);
 
+/* A x = b for symmetric A that may be indefinite or singular: MINRES (Paige & Saunders, SINUM 12, 1975),
+ * unpreconditioned, in the formulation of scipy.sparse.linalg.minres.  A is the operator the solver holds
+ * (with the eps it was built with); the product is the one the CG solvers use.  b and x are host vectors as
+ * in acgsolvercuda_solvempi, x the initial guess on entry and the solution on return.  Stopping rule as
+ * acgsolvercuda_solvempi: tol = threshold(atol, rtol, ||r0||), the strict test phi-bar < tol on MINRES's
+ * recursively updated residual norm phi-bar, 0 iterations if ||r0|| meets it, ACG_ERR_NOT_CONVERGED by the
+ * same rule.  The loop also ends, whatever the tolerance, on an exact Krylov breakdown beta_{k+1} = 0 (after
+ * that iteration's update: x is then the minimal-residual solution over an invariant subspace) and on
+ * gamma_k = 0, possible only for singular A (before that iteration's update, which is not counted).
+ * ||r0|| = 0 runs no iteration; maxits = 0 returns x0 unchanged.  One GPU, unpartitioned matrix: ghost
+ * rows or a communicator of more than one rank give ACG_ERR_NOT_SUPPORTED.  In *cg: niterations,
+ * bnrm2, r0nrm2, rnrm2 (the final phi-bar), the times and the counters, as for any solve.  `warmup`
+ * iterations run first on scratch state; the results do not depend on them. */
+ACG_API int acgsolvercuda_solve_minres(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A,
+                                       const struct acgvector *b, struct acgvector *x, int maxits,
+                                       double residualatol, double residualrtol, int warmup, int *errcode);
+
 struct acgb200_info {
     int spmv_lanes_per_row, spmv_rows_cap, spmv_nnz_cap, spmv_stages;
     int spmv_ntiles, spmv_nlong, spmv_grid, spmv_smem_bytes;
