@@ -130,7 +130,8 @@ class acgb200_info(C.Structure):
         [("spmv_slice_value_bytes", C.c_int64), ("spmv_slice_nnz", C.c_int64)] + \
         [("spmv_symdiag_diagonals", C.c_int), ("spmv_symdiag_bytes", C.c_int64)] + \
         [("pcg_fused", C.c_int), ("pcg_fused_min_bytes", C.c_int64)] + \
-        [("spmv_symdiag_codes", C.c_int), ("spmv_symdiag_code_bytes", C.c_int64)]
+        [("spmv_symdiag_codes", C.c_int), ("spmv_symdiag_code_bytes", C.c_int64)] + \
+        [("mixed_reliable_updates", C.c_int)]
 
 
 class acgb200_colstats(C.Structure):
@@ -162,7 +163,7 @@ EXPORTS = [
     "acgsolvercuda_init_constants", "acgsolvercuda_alpha", "acgsolvercuda_beta", "acgsolvercuda_daxpy_alpha",
     "acgsolvercuda_daxpy_minus_alpha", "acgsolvercuda_daypx_beta", "acgsolvercuda_pipelined_daxpy_fused",
     "acgsolvercuda_fwrite",
-    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_solve_multi", "acgsolvercuda_spmm_mode", "acgsolvercuda_solve_shifted", "acgsolvercuda_solve_minres", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
+    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_solve_multi", "acgsolvercuda_spmm_mode", "acgsolvercuda_solve_shifted", "acgsolvercuda_solve_minres", "acgsolvercuda_solve_mixed", "acgsolvercuda_spmv_f32", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
     "acgb200_nccl_unique_id", "acgb200_comm_init_rank", "acgb200_comm_destroy",
     "acgb200_host_register", "acgb200_host_unregister", "acgb200_spmv_plan_host", "acgb200_spmv_plan_host2", "acgb200_slices_host", "acgb200_symdiag_host", "acgb200_merge_plan_host", "acgb200_p2p_inverse_map", "acgb200_patterns_host", "acgb200_stencil_part",
     "acgb200_mtx_info", "acgb200_mtx_read", "acgb200_mtx_read_part", "acgb200_comm_matrix_row", "acgb200_partition_rows_grid", "acgb200_grid_factors", "acgb200_rmat_spd",
@@ -248,6 +249,10 @@ def lib() -> C.CDLL:
                                               C.c_double, C.c_double, C.c_int, P(acgb200_colstats)]
     L.acgsolvercuda_solve_minres.argtypes = [P(acgsolvercuda), P(acgsymcsrmatrix), P(acgvector), P(acgvector), C.c_int,
                                              C.c_double, C.c_double, C.c_int, P(C.c_int)]
+    L.acgsolvercuda_solve_mixed.argtypes = [P(acgsolvercuda), P(acgsymcsrmatrix), P(acgvector), P(acgvector), C.c_int,
+                                            C.c_double, C.c_double, C.c_int, P(C.c_int)]
+    f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
+    L.acgsolvercuda_spmv_f32.argtypes = [P(acgsolvercuda), f32p, f32p, P(C.c_double)]
     L.acgsolvercuda_info.argtypes = [P(acgsolvercuda), P(acgb200_info)]
     L.acgb200_set_option.argtypes = [C.c_char_p, C.c_int]
     L.acgb200_nccl_unique_id.argtypes = [C.c_void_p]
@@ -802,6 +807,32 @@ class SolverCuda:
         if code != ACG_SUCCESS and (raise_on_not_converged or code != ACG_ERR_NOT_CONVERGED):
             raise AcgError(code, "acgsolvercuda_solve_minres", err.value)
         return code
+
+    def solve_mixed(self, b, x, maxits=100, residualatol=0.0, residualrtol=0.0, warmup=0,
+                    raise_on_not_converged=False):
+        """acgsolvercuda_solve_mixed: CG with float vectors and reliable updates to an fp64 tolerance on
+        the solver's (positive definite) operator (one GPU, whole matrix).  b, x: Vectors as for
+        ``solvempi``, x the initial guess, updated in place.  ``c.rnrm2`` is the fp64 residual of the x
+        returned; ``info()["mixed_reliable_updates"]`` counts the reliable updates.  Returns the code like
+        ``solve()``."""
+        err = C.c_int(0)
+        code = lib().acgsolvercuda_solve_mixed(C.byref(self.c), C.byref(self.A.c), C.byref(b.c), C.byref(x.c),
+                                               int(maxits), float(residualatol), float(residualrtol), int(warmup),
+                                               C.byref(err))
+        if code != ACG_SUCCESS and (raise_on_not_converged or code != ACG_ERR_NOT_CONVERGED):
+            raise AcgError(code, "acgsolvercuda_solve_mixed", err.value)
+        return code
+
+    def spmv_f32(self, x: np.ndarray):
+        """The fp32 product of solve_mixed (acgsolvercuda_spmv_f32): y = fl32(A x) for float32 x over the
+        owned rows, each row summed in fp64.  Returns (y as float32, the fp64 dot x.y)."""
+        no = self.A.c.nownedrows
+        x = np.ascontiguousarray(x, np.float32)
+        assert len(x) == no
+        y = np.zeros(no, np.float32)
+        dot = C.c_double(0)
+        _check(lib().acgsolvercuda_spmv_f32(C.byref(self.c), x, y, C.byref(dot)), "acgsolvercuda_spmv_f32")
+        return y, dot.value
 
     def spmm_mode(self, mode: int, X: np.ndarray, B: np.ndarray | None = None):
         """The multi-vector product of solve_multi in one of the epilogue modes (acgsolvercuda_spmm_mode):

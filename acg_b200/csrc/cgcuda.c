@@ -171,10 +171,11 @@ struct priv {
     struct acgcomm redcomm;             /* private duplicate of the caller's communicator for reductions */
     int have_redcomm;
     double *d_b, *d_x;                  /* right-hand side / solution on the device, kept between solves */
-    cudaGraphExec_t graph[5];           /* [0] classic, [1] pipelined, [2] several right-hand sides, [3] shifted
-                                         * systems, [4] MINRES: two iterations each (parity 0 then 1) */
-    int graph_sig[5];                   /* loop configuration each cached graph was captured with (graph_signature) */
-    int graph_launches[5];              /* kernel/NCCL launches inside one replay */
+    cudaGraphExec_t graph[6];           /* [0] classic, [1] pipelined, [2] several right-hand sides, [3] shifted
+                                         * systems, [4] MINRES, [5] mixed precision: two iterations each (parity 0
+                                         * then 1) */
+    int graph_sig[6];                   /* loop configuration each cached graph was captured with (graph_signature) */
+    int graph_launches[6];              /* kernel/NCCL launches inside one replay */
     double last_h2d_ms, last_d2h_ms;    /* host time spent before / after the solve window */
     cudaEvent_t ev_t0, ev_t1;           /* device-side bracket of the solve window */
     double last_solve_ms;
@@ -198,6 +199,14 @@ struct priv {
      * (v lives in d_r / d_p, t and u in d_t) */
     struct acgb200_nstate *d_ns, *h_ns;
     double *d_nw[2];
+    /* mixed precision (acgsolvercuda_solve_mixed), made at the first such solve: its scalars, the float
+     * vectors r, p, t, y (one allocation; the fp64 residual lives in d_r) and the row chunks of its product
+     * outside the mirrored diagonals */
+    struct acgb200_xstate *d_xs, *h_xs;
+    float *d_f32;
+    int *d_franges;
+    int nfranges, have_franges;
+    int last_mixed_updates;
 };
 
 /* The public struct has no room for private state (its layout is the
@@ -286,7 +295,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
             pv->p2p.window = NULL;
         }
         if (pv->have_redcomm && pv->redcomm.ncclcomm) ncclCommDestroy(pv->redcomm.ncclcomm);
-        for (int i = 0; i < 5; i++) if (pv->graph[i]) cudaGraphExecDestroy(pv->graph[i]);
+        for (int i = 0; i < 6; i++) if (pv->graph[i]) cudaGraphExecDestroy(pv->graph[i]);
         cudaFree(pv->plan.d_tiles); cudaFree(pv->plan.d_longrows); cudaFree(pv->plan.d_long_scratch); cudaFree(pv->plan.d_medrows);
         cudaFree(pv->plan.d_slices); cudaFree(pv->plan.d_sval); cudaFree(pv->plan.d_spatoff); cudaFree(pv->plan.d_spatid);
         cudaFree(pv->plan.d_hval); cudaFree(pv->plan.d_symdiag_bad); cudaFree(pv->plan.d_hcode); cudaFree(pv->plan.d_codes);
@@ -301,6 +310,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
         cudaFree(pv->d_ms); cudaFreeHost(pv->h_ms); cudaFree(pv->d_ranges);
         cudaFree(pv->d_ss); cudaFreeHost(pv->h_ss);
         cudaFree(pv->d_ns); cudaFreeHost(pv->h_ns); cudaFree(pv->d_nw[0]); cudaFree(pv->d_nw[1]);
+        cudaFree(pv->d_xs); cudaFreeHost(pv->h_xs); cudaFree(pv->d_f32); cudaFree(pv->d_franges);
         cudaFree(pv->d_mx); cudaFree(pv->d_mb); cudaFree(pv->d_mr); cudaFree(pv->d_mp); cudaFree(pv->d_mt);
         if (pv->ev_ready) cudaEventDestroy(pv->ev_ready);
         if (pv->ev_halo) cudaEventDestroy(pv->ev_halo);
@@ -889,6 +899,7 @@ struct solvectx {
     int mk;                   /* multi-vector loop: block width K (0: single vector) */
     int shifted;              /* shifted-systems loop (acgsolvercuda_solve_shifted) */
     int minres;               /* MINRES loop (acgsolvercuda_solve_minres) */
+    int mixed;                /* mixed-precision loop (acgsolvercuda_solve_mixed) */
     int fused;                /* pipelined loop: one fused iteration (acgb200_pcg_fused_launch); its control word
                                * alternates between ctrl[0] and ctrl[1] by iteration parity */
     int issued;               /* iterations iterate() issued, inactive ones included */
@@ -931,7 +942,9 @@ static void offdiag_epilogue(struct acgb200_offdiagargs *o, int mode)
 
 /* y = A x (or r = b - A x) over owned rows, including the halo exchange of x
  * and the border x ghost block when the matrix is distributed.  `acc` gets the
- * fused dot.  `gated`: take part in the device-side iteration control. */
+ * fused dot.  `gated`: take part in the device-side iteration control; 2: only
+ * run when ctrl[2] is active, passing nothing on (the mixed-precision loop's
+ * reliable update; the tile kernel's copy of the word goes to ctrl[3]). */
 static int apply_A(struct solvectx *c, const double *x_ro, double *x_halo, double *y, const double *b,
                    int mode, double *acc, int gated, int housekeeping, int warmup, int pub_ch)
 {
@@ -956,7 +969,8 @@ static int apply_A(struct solvectx *c, const double *x_ro, double *x_halo, doubl
     a.x = x_ro; a.y = y; a.b = b; a.acc = acc;
     a.dotrows = (c->multi && !peer) ? pv->borderoff : pv->nowned;
     a.mode = mode;
-    if (gated) { a.ctrl_in = &pv->d_st->ctrl[0]; a.ctrl_out = &pv->d_st->ctrl[1]; }
+    if (gated == 2) { a.ctrl_in = &pv->d_st->ctrl[2]; a.ctrl_out = &pv->d_st->ctrl[3]; }
+    else if (gated) { a.ctrl_in = &pv->d_st->ctrl[0]; a.ctrl_out = &pv->d_st->ctrl[1]; }
     a.st = pv->d_st; a.housekeeping = housekeeping;
     a.pub_ch = -1;
     const int fused = peer && pv->p2p.h_desc.fuse;
@@ -1131,7 +1145,7 @@ static int graph_signature(const struct solvectx *c)
 {
     return 1 | (c->multi ? 2 : 0) | (c->p2p ? 4 : 0) | (c->pv->p2p.h_desc.fuse ? 8 : 0) | (cfg.pdl ? 16 : 0)
            | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0) | (c->shifted ? 128 : 0) | (c->mk << 8)
-           | (c->fused ? 1 << 16 : 0) | (c->minres ? 1 << 17 : 0);
+           | (c->fused ? 1 << 16 : 0) | (c->minres ? 1 << 17 : 0) | (c->mixed ? 1 << 18 : 0);
 }
 
 static int capture_pair(struct solvectx *c, int kind, int (*issue)(struct solvectx *, int))
@@ -1396,10 +1410,11 @@ static int block_width(int nrhs) { return nrhs <= 1 ? 1 : nrhs <= 2 ? 2 : nrhs <
  * plan (its slices; every other row -- tile, merge, medium, long -- goes to the chunks).  Lanes per row
  * from the mean length of those rows. */
 #define SPMM_CHUNK_LANES 128
-static int build_ranges(struct priv *pv, const struct acgsolvercuda *cg, int *errcode)
+/* (all rows if !use_slices: the fp32 product of a plan without mirrored diagonals) */
+static int row_chunks(struct priv *pv, const struct acgsolvercuda *cg, int use_slices, int **d_out, int *nr_out,
+                      int *lanes_out, int *errcode)
 {
-    if (pv->have_ranges) return ACG_SUCCESS;
-    const int n = pv->nowned, nsl = pv->plan.nslices;
+    const int n = pv->nowned, nsl = use_slices ? pv->plan.nslices : 0;
     unsigned char *cov = calloc((size_t) n + 1, 1);
     int *rp = malloc(((size_t) n + 1) * sizeof(int));
     struct acgb200_slice *sl = nsl > 0 ? malloc((size_t) nsl * sizeof(*sl)) : NULL;
@@ -1422,12 +1437,20 @@ static int build_ranges(struct priv *pv, const struct acgsolvercuda *cg, int *er
         rg[2 * nr] = r0; rg[2 * nr + 1] = r; nr++;
     }
     if (nr > 0) {
-        e = cudaMalloc((void **) &pv->d_ranges, (size_t) nr * 2 * sizeof(int));
-        if (!e) e = cudaMemcpy(pv->d_ranges, rg, (size_t) nr * 2 * sizeof(int), cudaMemcpyHostToDevice);
+        e = cudaMalloc((void **) d_out, (size_t) nr * 2 * sizeof(int));
+        if (!e) e = cudaMemcpy(*d_out, rg, (size_t) nr * 2 * sizeof(int), cudaMemcpyHostToDevice);
     }
     free(cov); free(rp); free(sl); free(rg);
     CU(e);
-    pv->nranges = nr; pv->ranges_lanes = lanes; pv->have_ranges = 1;
+    *nr_out = nr; *lanes_out = lanes;
+    return ACG_SUCCESS;
+}
+
+static int build_ranges(struct priv *pv, const struct acgsolvercuda *cg, int *errcode)
+{
+    if (pv->have_ranges) return ACG_SUCCESS;
+    OK(row_chunks(pv, cg, 1, &pv->d_ranges, &pv->nranges, &pv->ranges_lanes, errcode));
+    pv->have_ranges = 1;
     return ACG_SUCCESS;
 }
 
@@ -2068,6 +2091,265 @@ int acgsolvercuda_solve_minres(struct acgsolvercuda *cg, const struct acgsymcsrm
 }
 
 /* ------------------------------------------------------------------------ */
+/* mixed-precision CG with reliable updates                                  */
+/* ------------------------------------------------------------------------ */
+
+/* the mixed-precision kernels are linked in (see ACGB200_MULTI_LAUNCHER, internal.h) */
+static int have_mixed_kernels(void)
+{
+    return acgb200_spmv_f32_launch && acgb200_mixed_setup && acgb200_mixed_update_r && acgb200_mixed_update_yp
+           && acgb200_mixed_replace && acgb200_mixed_fold;
+}
+
+/* the float vectors (16 bytes per row), the scalars and the product's row chunks, made once per solver */
+static int mixed_alloc(struct priv *pv, const struct acgsolvercuda *cg, int *errcode)
+{
+    if (!pv->d_xs) {
+        CU(cudaMalloc((void **) &pv->d_xs, sizeof(*pv->d_xs)));
+        CU(cudaMallocHost((void **) &pv->h_xs, sizeof(*pv->h_xs)));
+    }
+    if (!pv->d_f32) {
+        /* four vectors of nowned + 2 floats, each starting on an 8-byte boundary (the kernels read pairs) */
+        const size_t bytes = 4 * (((size_t) pv->nowned + 2) & ~(size_t) 1) * sizeof(float);
+        CU(cudaMalloc((void **) &pv->d_f32, bytes));
+        CU(cudaMemset(pv->d_f32, 0, bytes));
+    }
+    if (!pv->have_franges) {
+        int lanes = 0;
+        OK(row_chunks(pv, cg, pv->plan.symdiag_nd > 0, &pv->d_franges, &pv->nfranges, &lanes, errcode));
+        pv->have_franges = 1;
+    }
+    return ACG_SUCCESS;
+}
+
+static float *mixed_vec(const struct priv *pv, int i)     /* 0 r, 1 p, 2 t, 3 y */
+{
+    return pv->d_f32 + (size_t) i * (((size_t) pv->nowned + 2) & ~(size_t) 1);
+}
+
+static int push_xstate(struct solvectx *c, const struct acgb200_xstate *xs)
+{
+    int *errcode = c->errcode;
+    CU(cudaStreamSynchronize(c->pv->stream));
+    *c->pv->h_xs = *xs;
+    CU(cudaMemcpyAsync(c->pv->d_xs, c->pv->h_xs, sizeof(*xs), cudaMemcpyHostToDevice, c->pv->stream));
+    CU(cudaStreamSynchronize(c->pv->stream));
+    return ACG_SUCCESS;
+}
+
+static int pull_xstate(struct solvectx *c, struct acgb200_xstate *xs)
+{
+    int *errcode = c->errcode;
+    CU(cudaMemcpyAsync(c->pv->h_xs, c->pv->d_xs, sizeof(*xs), cudaMemcpyDeviceToHost, c->pv->stream));
+    CU(cudaStreamSynchronize(c->pv->stream));
+    *xs = *c->pv->h_xs;
+    return ACG_SUCCESS;
+}
+
+/* the fp32 product t = fl32(A p) with (p, t) into acc; gated: by ctrl[0] */
+static int apply_A_f32(struct solvectx *c, const float *x, float *y, double *acc, int gated)
+{
+    struct acgsolvercuda *cg = c->cg;
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    struct acgb200_spmvf32args a;
+    memset(&a, 0, sizeof(a));
+    a.plan = &pv->plan;
+    a.nranges = pv->nfranges; a.ranges = pv->d_franges;
+    a.rowptr = cg->d_rowptr; a.colidx = cg->d_colidx; a.a = cg->d_a;
+    a.x = x; a.y = y; a.acc = acc;
+    a.ctrl_in = gated ? &pv->d_st->ctrl[0] : NULL; a.st = pv->d_st;
+    prof_mark(c, &pv->gemv);
+    KL(acgb200_spmv_f32_launch(&a, pv->stream));
+    prof_mark(c, &pv->gemv);
+    c->launches += (pv->plan.nslices > 0 && pv->plan.symdiag_nd > 0) + (pv->nfranges > 0);
+    return ACG_SUCCESS;
+}
+
+/* r64 = b - A x into d_r with (r64, r64) folded in (ungated) */
+static int mixed_residual(struct solvectx *c, double *rr)
+{
+    struct priv *pv = c->pv;
+    struct acgb200_devstate h;
+    memset(&h, 0, sizeof(h));
+    OK(push_state(c, &h));
+    *rr = 0;
+    OK(apply_A(c, c->d_x, c->d_x, c->cg->d_r, c->d_b, SPMV_R_B_AX, &pv->d_st->tmp_loc[0], 0, 0, 0, -1));
+    return reduce_to_host(c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, rr);
+}
+
+/* sigma = 2^round(log2 sqrt(rr)) as its exponent (as mixed_scale_exp of kernels.cu) */
+static int mixed_scale_exp(double rr)
+{
+    int e = 0;
+    const double m = frexp(sqrt(rr), &e);
+    return m < 0.70710678118654752440 ? e - 1 : e;
+}
+
+/* r = fl32(r64 / sigma), p = r, y = 0 and the scalars of the first iteration; rr64 = (r64, r64) > 0 */
+static int mixed_start(struct solvectx *c, int maxits, double tol, double rr64)
+{
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    const int e = mixed_scale_exp(rr64);
+    KL(acgb200_mixed_setup(pv->nowned, ldexp(1.0, -e), c->cg->d_r, mixed_vec(pv, 0), mixed_vec(pv, 1), mixed_vec(pv, 3),
+                           pv->stream));
+    c->launches += 1;
+    struct acgb200_xstate xs;
+    memset(&xs, 0, sizeof(xs));
+    xs.rho[0] = ldexp(rr64, -2 * e); xs.mx[0] = sqrt(xs.rho[0]); xs.sigma[0] = ldexp(1.0, e);
+    xs.last_rr64 = rr64;
+    OK(push_xstate(c, &xs));
+    struct acgb200_devstate h;
+    memset(&h, 0, sizeof(h));
+    h.maxits = maxits; h.tol = tol;
+    return push_state(c, &h);
+}
+
+/* iteration k: t = fl32(A p) (+ pi), r -= alpha t (+ rho'), y and p (or the fold), the fp64 residual and
+ * the replacement -- the last two idle unless a reliable update is due */
+static int mixed_iteration(struct solvectx *c, int k)
+{
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    const int s = k & 1, n = pv->nowned;
+    float *r = mixed_vec(pv, 0), *p = mixed_vec(pv, 1), *t = mixed_vec(pv, 2), *y = mixed_vec(pv, 3);
+    OK(apply_A_f32(c, p, t, &pv->d_xs->pi[s], 1));
+    prof_mark(c, &pv->blas);
+    KL(acgb200_mixed_update_r(n, pv->d_st, pv->d_xs, t, r, pv->stream));
+    KL(acgb200_mixed_update_yp(n, pv->d_st, pv->d_xs, r, p, y, c->d_x, pv->stream));
+    prof_mark(c, &pv->blas);
+    OK(apply_A(c, c->d_x, c->d_x, c->cg->d_r, c->d_b, SPMV_R_B_AX, &pv->d_xs->rr64[s], 2, 0, 0, -1));
+    KL(acgb200_mixed_replace(n, pv->d_st, pv->d_xs, c->cg->d_r, r, p, pv->stream));
+    c->launches += 3;
+    return ACG_SUCCESS;
+}
+
+static void account_mixed(struct acgsolvercuda *cg, const struct priv *pv, int nits, int nupdates)
+{
+    /* per iteration: the product on float vectors (4-byte gathers and store) with (p, t) folded in, then
+     * update_r (12 bytes per row) and update_yp (20); each reliable update adds an fp64 residual product
+     * and the replacement (20 bytes per row) */
+    const int64_t n = pv->nowned, nnz = pv->fnnz + pv->onnz;
+    cg->ngemv += nits + nupdates; cg->nflops += (int64_t) (nits + nupdates) * 3 * nnz;
+    cg->Bgemv += (int64_t) nits * (nnz * 12 + n * 12) + (int64_t) nupdates * (nnz * 12 + n * 24);
+    cg->ndot += nits; cg->nflops += (int64_t) nits * 2 * n; cg->Bdot += (int64_t) nits * 8 * n;
+    cg->nnrm2 += nits; cg->nflops += (int64_t) nits * 2 * n; cg->Bnrm2 += (int64_t) nits * 4 * n;
+    cg->naxpy += 3 * (int64_t) nits; cg->nflops += (int64_t) nits * 6 * n; cg->Baxpy += (int64_t) nits * 32 * n;
+}
+
+int acgsolvercuda_solve_mixed(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A,
+                              const struct acgvector *b, struct acgvector *x, int maxits,
+                              double residualatol, double residualrtol, int warmup, int *errcode)
+{
+    int errcode_ = 0;
+    if (!errcode) errcode = &errcode_;
+    cfg_load();
+    struct priv *pv = priv_of(cg);
+    if (!pv || !A || !b || !x) return ACG_ERR_INVALID_VALUE;
+    if (!have_mixed_kernels() || pv->nghost > 0 || pv->commsize > 1 || A->nghostrows > 0)
+        return ACG_ERR_NOT_SUPPORTED;      /* one GPU, whole matrix */
+    if (maxits < 0) return ACG_ERR_INVALID_VALUE;
+    struct acgcomm null;
+    memset(&null, 0, sizeof(null));
+    null.type = acgcomm_null;
+    struct solvectx c;
+    OK(solve_begin(&c, cg, A, b, x, 0.0, 0.0, &null, 0, errcode));
+    c.mixed = 1;
+    const int n = pv->nowned;
+    OK(mixed_alloc(pv, cg, errcode));
+    struct acgb200_devstate h;
+    struct acgb200_xstate xs;
+
+    /* warm-up: the set-up and `warmup` iterations on x itself, then x0 again from the caller's vector */
+    if (warmup > 0) {
+        double rr = 0;
+        OK(mixed_residual(&c, &rr));
+        if (rr > 0) {
+            OK(mixed_start(&c, warmup, 0.0, rr));
+            for (int i = 0; i < warmup; i++) OK(mixed_iteration(&c, i));
+        }
+        const double tb = wall();
+        const size_t nx = (size_t) (x->num_nonzeros < pv->nvec ? x->num_nonzeros : pv->nvec);
+        CU(cudaMemcpyAsync(c.d_x, x->x, nx * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
+        CU(cudaStreamSynchronize(pv->stream));
+        pv->last_h2d_ms += 1e3 * (wall() - tb);
+    }
+    if (cfg.profile) {
+        OK(evpool_reserve(&pv->gemv, 2 * (maxits + 2)));
+        OK(evpool_reserve(&pv->blas, 2 * (maxits + 2)));
+    }
+    pv->gemv.n = pv->blas.n = 0;
+
+    cg->nsolves++; cg->niterations = 0;
+    cg->bnrm2 = cg->r0nrm2 = cg->rnrm2 = cg->x0nrm2 = cg->dxnrm2 = INFINITY;
+    cg->maxits = maxits; cg->diffatol = 0; cg->diffrtol = 0;
+    cg->residualatol = residualatol; cg->residualrtol = residualrtol;
+    pv->last_mixed_updates = 0;
+    CU(cudaStreamSynchronize(pv->stream));
+    const double t0 = wall();
+    CU(cudaEventRecord(pv->ev_t0, pv->stream));
+    c.launches = 0;
+
+    /* ||b|| ; r0 = b - A x0 in fp64 */
+    memset(&h, 0, sizeof(h));
+    OK(push_state(&c, &h));
+    double bb = 0, rr0 = 0;
+    KL(acgb200_dot(n, c.d_b, c.d_b, &pv->d_st->tmp_loc[0], pv->stream));
+    OK(reduce_to_host(&c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &bb));
+    c.launches += 1;
+    cg->bnrm2 = sqrt(bb);
+    OK(mixed_residual(&c, &rr0));
+    cg->rnrm2 = cg->r0nrm2 = sqrt(rr0);
+    cg->nnrm2 += 2; cg->nflops += 4 * (int64_t) n; cg->Bnrm2 += 8 * (int64_t) n; cg->ngemv++;
+    const double tol = threshold(residualatol, residualrtol, cg->r0nrm2);
+    const double rtol_scaled = residualrtol * cg->r0nrm2;
+    int converged = tol > 0 && cg->rnrm2 < tol;                    /* acg/cgcuda.c:836-842 */
+    int nupdates = 0;
+
+    /* ||r0|| = 0: x0 solves the system */
+    if (!converged && maxits > 0 && rr0 > 0) {
+        OK(mixed_start(&c, maxits, tol, rr0));
+        OK(iterate(&c, maxits, 1, 5, mixed_iteration));
+        OK(pull_state(&c, &h));
+        OK(pull_xstate(&c, &xs));
+        cg->niterations = h.ctrl[0].iter;
+        nupdates = xs.nupdates;
+        if (xs.conv || xs.breakdown) {
+            /* y was folded into x (or is dropped: a breakdown returns the last fold), whose residual is known */
+            cg->rnrm2 = sqrt(xs.last_rr64);
+        } else {
+            /* maxits: the last fold, then the residual of the x returned */
+            KL(acgb200_mixed_fold(n, xs.sigma[cg->niterations & 1], mixed_vec(pv, 3), c.d_x, pv->stream));
+            double rr = 0;
+            OK(mixed_residual(&c, &rr));
+            c.launches += 1;
+            cg->rnrm2 = sqrt(rr);
+            cg->ngemv++;
+        }
+        converged = tol > 0 && cg->rnrm2 < tol;
+        cg->ntotaliterations += cg->niterations;
+    }
+    CU(cudaEventRecord(pv->ev_t1, pv->stream));
+    CU(cudaEventSynchronize(pv->ev_t1));
+    cg->tsolve += wall() - t0;
+    { float ms = 0; if (cudaEventElapsedTime(&ms, pv->ev_t0, pv->ev_t1) == cudaSuccess) pv->last_solve_ms = ms; }
+    account_mixed(cg, pv, cg->niterations, nupdates);
+    pv->last_launches = c.launches;
+    pv->last_fused = 0;
+    pv->last_mixed_updates = nupdates;
+    if (cfg.profile) {
+        pv->last_spmv_ms = evpool_sum_ms(&pv->gemv); pv->last_spmv_n = pv->gemv.n / 2;
+        pv->last_blas_ms = evpool_sum_ms(&pv->blas);
+        cg->tgemv += 1e-3 * pv->last_spmv_ms;
+        cg->taxpy += 1e-3 * pv->last_blas_ms;
+    }
+    int status = ACG_SUCCESS;
+    if (!converged && !(residualatol == 0 && rtol_scaled == 0)) status = ACG_ERR_NOT_CONVERGED;   /* :1099-1107 */
+    return solve_end(&c, x, status);
+}
+
+/* ------------------------------------------------------------------------ */
 /* pipelined CG                                                              */
 /* ------------------------------------------------------------------------ */
 
@@ -2588,6 +2870,33 @@ int acgsolvercuda_spmv_mode(struct acgsolvercuda *cg, int mode, const double *x,
     return ACG_SUCCESS;
 }
 
+/* The fp32 product of acgsolvercuda_solve_mixed on host float vectors: y = fl32(A x) over the owned rows
+ * (x: nowned floats), *dot = (x, y) in fp64.  y is poisoned on the device first, so a row no kernel writes
+ * reads NaN. */
+int acgsolvercuda_spmv_f32(struct acgsolvercuda *cg, const float *x, float *y, double *dot)
+{
+    int errcode_ = 0, *errcode = &errcode_;
+    struct priv *pv = priv_of(cg);
+    if (!pv || !x || !y) return ACG_ERR_INVALID_VALUE;
+    if (!have_mixed_kernels() || pv->nghost > 0 || pv->commsize > 1) return ACG_ERR_NOT_SUPPORTED;
+    OK(mixed_alloc(pv, cg, errcode));
+    const int n = pv->nowned;
+    struct acgb200_devstate *st = pv->d_st;
+    CU(cudaMemcpyAsync(mixed_vec(pv, 1), x, (size_t) n * sizeof(float), cudaMemcpyHostToDevice, pv->stream));
+    CU(cudaMemsetAsync(mixed_vec(pv, 2), 0xff, (size_t) n * sizeof(float), pv->stream));
+    CU(cudaMemsetAsync(&st->tmp_loc[0], 0, sizeof(double), pv->stream));
+    struct solvectx c;
+    memset(&c, 0, sizeof(c));
+    c.cg = cg; c.pv = pv; c.errcode = errcode;
+    OK(apply_A_f32(&c, mixed_vec(pv, 1), mixed_vec(pv, 2), &st->tmp_loc[0], 0));
+    double hdot = 0;
+    CU(cudaMemcpyAsync(y, mixed_vec(pv, 2), (size_t) n * sizeof(float), cudaMemcpyDeviceToHost, pv->stream));
+    CU(cudaMemcpyAsync(&hdot, &st->tmp_loc[0], sizeof(double), cudaMemcpyDeviceToHost, pv->stream));
+    CU(cudaStreamSynchronize(pv->stream));
+    if (dot) *dot = hdot;
+    return ACG_SUCCESS;
+}
+
 /* The multi-vector product of acgsolvercuda_solve_multi in any of the three epilogue modes, for
  * nrhs columns (padded to the block width K as the solver pads them): X, B (mode 2) and Y are host
  * arrays of nowned x nrhs doubles, row-major; dots[j] gets column j's fused dot.  Y is poisoned on
@@ -2658,5 +2967,6 @@ int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info
     info->pcg_fused_min_bytes = pv->plan.symdiag_nd > 0 ? acgb200_pcg_fused_min_bytes(&pv->plan) : 0;
     info->spmv_symdiag_codes = pv->plan.symdiag_codes;
     info->spmv_symdiag_code_bytes = pv->plan.symdiag_codes > 0 ? (int64_t) pv->plan.symdiag_nd * pv->plan.symdiag_stride : 0;
+    info->mixed_reliable_updates = pv->last_mixed_updates;
     return ACG_SUCCESS;
 }

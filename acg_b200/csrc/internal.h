@@ -524,6 +524,67 @@ ACGB200_MULTI_LAUNCHER int acgb200_minres_update(int n, struct acgb200_devstate 
                                                  int cin, int cout, const double *v, const double *u, double *w,
                                                  const double *wprev, double *x, double *vnext, cudaStream_t stream);
 
+/* ------------------------------------------------------------------------
+ * Mixed-precision CG with reliable updates (acgsolvercuda_solve_mixed): r, p,
+ * t and y are float vectors scaled by an exact power of two sigma; every
+ * operation is fp64 and each stored value is rounded once.  x and b stay fp64.
+ * Iteration k (parity s = k&1) runs five steps:
+ *   1. t = fl32(A p), pi = (p, t) into pi[s]                 reads ctrl[0]
+ *   2. r = fl32(r - alpha t), (r,r) into rr[s]               reads ctrl[0]
+ *   3. y = fl32(y + alpha p); not due: p = fl32(r + beta p); due: x += sigma y,
+ *      y = 0.  Block 0 writes ctrl[1] (the word after the iteration when no
+ *      update is due) and ctrl[2] (active only when one is due)  reads ctrl[0]
+ *   4. r64 = b - A x with (r64,r64) into rr64[s]: the fp64 product, gated by
+ *      ctrl[2] (its tile kernel copies the word into ctrl[3], read by nobody)
+ *   5. the replacement: rescale r and p from r64, the convergence test, and
+ *      ctrl[0] for the next iteration (ctrl[1] when no update was due)
+ * Slot s holds the scalars iteration k reads; block 0 of step 3 or 5 writes
+ * slot s^1 and zeroes its accumulators, so no kernel reads a slot it writes.
+ * ------------------------------------------------------------------------ */
+struct acgb200_xstate {
+    double pi[2];                    /* (p, A p) of the fp32 product */
+    double rr[2];                    /* rho' = (r, r) after update_r */
+    double rr64[2];                  /* (r64, r64) of a reliable update's fp64 residual */
+    double rho[2];                   /* rho_k = (r_k, r_k), scaled by 1/sigma^2 */
+    double mx[2];                    /* M: the largest sqrt(rho) since the last reliable update */
+    double sigma[2];                 /* the scale of the fp32 vectors (a power of two) */
+    double last_rr64;                /* (r64, r64) of the x of the last fold (x0 at set-up) */
+    int nupdates;                    /* reliable updates of the solve */
+    int conv;                        /* 1: a reliable update met the tolerance (or r64 = 0) */
+    int breakdown;                   /* 1: pi = 0 or non-finite ended the solve */
+    int pad;
+};
+/* the product t = fl32(A p) on float vectors: mirrored-diagonal rows through spmv_symdiag_kernel (float
+ * gathers and store), every other row through a CSR rows kernel over `ranges`, one thread per row in CSR
+ * order; acc += (p, t) over all rows if acc.  ctrl_in may be NULL (ungated). */
+struct acgb200_spmvf32args {
+    const struct acgb200_spmvplan *plan;  /* its mirrored diagonals, if symdiag_nd > 0 */
+    int nranges;                          /* row chunks the diagonals do not cover */
+    const int *ranges;                    /* [2 * nranges]: first row, one past the last row */
+    const int *rowptr, *colidx;
+    const double *a;
+    const float *x;
+    float *y;
+    double *acc;
+    const struct acgb200_ctrl *ctrl_in;
+    const struct acgb200_devstate *st;
+};
+ACGB200_MULTI_LAUNCHER int acgb200_spmv_f32_launch(const struct acgb200_spmvf32args *a, cudaStream_t stream);
+/* set-up: r = fl32(r64 * scale), p = r, y = 0 (scale = 1/sigma) */
+ACGB200_MULTI_LAUNCHER int acgb200_mixed_setup(int n, double scale, const double *r64, float *r, float *p, float *y,
+                                               cudaStream_t stream);
+/* step 2 (reads ctrl[0]) */
+ACGB200_MULTI_LAUNCHER int acgb200_mixed_update_r(int n, const struct acgb200_devstate *st, struct acgb200_xstate *xs,
+                                                  const float *t, float *r, cudaStream_t stream);
+/* step 3 (reads ctrl[0], writes ctrl[1] and ctrl[2]) */
+ACGB200_MULTI_LAUNCHER int acgb200_mixed_update_yp(int n, struct acgb200_devstate *st, struct acgb200_xstate *xs,
+                                                   const float *r, float *p, float *y, double *x, cudaStream_t stream);
+/* step 5 (reads ctrl[1] and ctrl[2], writes ctrl[0]) */
+ACGB200_MULTI_LAUNCHER int acgb200_mixed_replace(int n, struct acgb200_devstate *st, struct acgb200_xstate *xs,
+                                                 const double *r64, float *r, float *p, cudaStream_t stream);
+/* x += sigma y (the fold at maxits; ungated) */
+ACGB200_MULTI_LAUNCHER int acgb200_mixed_fold(int n, double sigma, const float *y, double *x, cudaStream_t stream);
+
 /* setup-time helpers */
 int acgb200_dot(int n, const double *x, const double *y, double *acc, cudaStream_t stream); /* acc += x.y */
 int acgb200_dot2(int n, const double *r, const double *w, double *acc2, cudaStream_t stream); /* acc2[0]+=r.r, acc2[1]+=w.r */

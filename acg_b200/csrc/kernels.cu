@@ -113,6 +113,14 @@ __device__ __forceinline__ double ld_x(const double *p)
     return v;
 }
 
+/* the same for a float vector (the fp32 product of the mixed-precision solve) */
+__device__ __forceinline__ float ld_x(const float *p)
+{
+    float v;
+    asm volatile("ld.global.nc.f32 %0, [%1];" : "=f"(v) : "l"(p));
+    return v;
+}
+
 /* coalesced read of matrix data that is used exactly once per SpMV: no L1 line, evict-first in L2,
  * so the stream does not displace the x vector (which every row re-reads) from either cache */
 __device__ __forceinline__ double ld_stream(const double *p, uint64_t pol)
@@ -820,15 +828,25 @@ struct SymdiagParams {
  * V: double reads the fp64 diagonals (hval); uint8_t reads one code per element (hcode) and decodes it from
  * a copy of the value table in shared memory just before the FMAs -- the same double, bit for bit, so the
  * same sums.  The codes of a batch are loaded with the values' L2 policy, 32 bytes per warp and entry.
+ *
+ * X: the vector type.  float (the mixed-precision solve, modes SPMV_Y_AX and SPMV_Y_AX_DOT only) gathers
+ * floats, widens them and runs the same fp64 FMA chain, then stores the sum rounded once to float; the
+ * fused dot is over (x_i, fl32(y_i)), products of two floats and so exact in fp64.
  */
+/* X = float: P.x and P.y hold the addresses of float vectors (the parameter block stays as it is) */
+template <typename X> __device__ __forceinline__ const X *sd_vec(const double *p) { return reinterpret_cast<const X *>(p); }
+template <typename X> __device__ __forceinline__ X *sd_vec(double *p) { return reinterpret_cast<X *>(p); }
+
 __device__ __forceinline__ double sd_decode(double v, const double *) { return v; }
 __device__ __forceinline__ double sd_decode(unsigned c, const double *vtab_s) { return vtab_s[c]; }
 
-template <int UB, int T, bool PCG, typename V>
+template <int UB, int T, bool PCG, typename V, typename X = double>
 __global__ void __launch_bounds__(T, PCG ? 1536 / T : 0)
 spmv_symdiag_kernel(const SymdiagParams P)
 {
     constexpr bool CODED = std::is_same<V, uint8_t>::value;
+    constexpr bool F32 = std::is_same<X, float>::value;
+    static_assert(!(F32 && PCG), "the fused pipelined-CG epilogue is fp64 only");
     typedef decltype(ld_stream((const V *) nullptr, 0)) R;      /* a loaded value or code */
     __shared__ int2 tab_s[ACGB200_SYMDIAG_MAX];
     __shared__ double vtab_s[CODED ? 256 : 1];
@@ -884,7 +902,7 @@ spmv_symdiag_kernel(const SymdiagParams P)
 #pragma unroll
             for (int u = 0; u < UB; u++) cv[u] = ld_stream(hv + tab_s[e + u].x, pol);
 #pragma unroll
-            for (int u = 0; u < UB; u++) xv[u] = ld_x(P.x + min(max(row + tab_s[e + u].y, 0), cmax));
+            for (int u = 0; u < UB; u++) xv[u] = ld_x(sd_vec<X>(P.x) + min(max(row + tab_s[e + u].y, 0), cmax));
 #pragma unroll
             for (int u = 0; u < UB; u++) vv[u] = sd_decode(cv[u], vtab_s);
             sum = slice_fma<UB>(vv, xv, sum);
@@ -896,7 +914,7 @@ spmv_symdiag_kernel(const SymdiagParams P)
 #pragma unroll
             for (int u = 0; u < UB; u++) cv[u] = e + u < L ? ld_stream(hv + tab_s[e + u].x, pol) : (R) 0;
 #pragma unroll
-            for (int u = 0; u < UB; u++) xv[u] = e + u < L ? ld_x(P.x + min(max(row + tab_s[e + u].y, 0), cmax)) : 0.0;
+            for (int u = 0; u < UB; u++) xv[u] = e + u < L ? ld_x(sd_vec<X>(P.x) + min(max(row + tab_s[e + u].y, 0), cmax)) : 0.0;
 #pragma unroll
             for (int u = 0; u < UB; u++) vv[u] = sd_decode(cv[u], vtab_s);
 #pragma unroll
@@ -905,6 +923,10 @@ spmv_symdiag_kernel(const SymdiagParams P)
         if (PCG) {
             /* w_i was gathered by this row a moment ago: an L1 hit, not a third stream */
             pcg_row(row, sum, __ldg(P.x + row), k, P.z, P.t, P.p, P.r, P.xs, P.w_next, vpol, dot, dot2);
+        } else if (F32) {
+            const X ys = (X) sum;
+            sd_vec<X>(P.y)[row] = ys;
+            if (P.mode == SPMV_Y_AX_DOT && row < P.dotrows) dot = fma((double) __ldg(sd_vec<X>(P.x) + row), (double) ys, dot);
         } else if (P.mode == SPMV_R_B_AX) {
             const double r = P.b[row] - sum;
             P.y[row] = r;
@@ -2381,6 +2403,231 @@ minres_update_kernel(int n, acgb200_devstate *st, acgb200_nstate *ns, int cin, i
     }
 }
 
+/* ---- mixed-precision CG with reliable updates ------------------------------------------------------- */
+
+/* The fp32 product's rows outside the mirrored diagonals (all rows without them): plain CSR, a warp per
+ * chunk of rows (the chunk list of spmm_rows_kernel), one thread per row summing (double) a_k * x[col_k]
+ * in CSR order into one fp64 accumulator, stored rounded once.  Correct on power-law rows, not tuned. */
+#define MIXED_ROWS_T 256
+__global__ void __launch_bounds__(MIXED_ROWS_T)
+spmv_rows_f32_kernel(int nranges, const int2 *__restrict__ ranges, const int *__restrict__ rowptr,
+                     const int *__restrict__ colidx, const double *__restrict__ a, const float *__restrict__ x,
+                     float *__restrict__ y, double *acc, const acgb200_ctrl *cin, const acgb200_devstate *st)
+{
+    __shared__ double red[MIXED_ROWS_T / 32];
+    pdl_prologue();
+    if (!gate_read(cin, st).active) return;
+    const int lane = threadIdx.x & 31;
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int nwarps = (gridDim.x * blockDim.x) >> 5;
+    double dot = 0.0;
+    for (int c = warp; c < nranges; c += nwarps) {
+        const int2 rg = ranges[c];
+        for (int row = rg.x + lane; row < rg.y; row += 32) {
+            double sum = 0.0;
+            const int ke = rowptr[row + 1];
+#pragma unroll 4
+            for (int k = rowptr[row]; k < ke; k++) sum = fma(__ldg(a + k), (double) ld_x(x + __ldg(colidx + k)), sum);
+            const float ys = (float) sum;
+            y[row] = ys;
+            dot = fma((double) __ldg(x + row), (double) ys, dot);
+        }
+    }
+    if (acc) {
+        const double v = block_sum(dot, red);
+        if (threadIdx.x == 0 && v != 0.0) atomicAdd(acc, v);
+    }
+}
+
+/* r = fl32(r64 * scale), p = r, y = 0 */
+__global__ void __launch_bounds__(BLAS1_THREADS)
+mixed_setup_kernel(int n, double scale, const double *__restrict__ r64, float *__restrict__ r, float *__restrict__ p,
+                   float *__restrict__ y)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const float v = (float) (r64[i] * scale);
+        r[i] = v; p[i] = v; y[i] = 0.0f;
+    }
+}
+
+/* The scalars of mixed iteration k from slot s; every thread of the update kernels derives them alike.
+ * pi = 0 or non-finite is a breakdown: the iteration does nothing and is not counted. */
+#define MIXED_DELTA 0.1
+struct MixedStep { double alpha, rr, beta; bool bad, due; };
+
+__device__ __forceinline__ MixedStep mixed_step(const acgb200_devstate *st, const acgb200_xstate *xs, int s)
+{
+    MixedStep o;
+    const double pi = xs->pi[s], rho = xs->rho[s];
+    o.bad = !(pi != 0.0 && isfinite(pi));
+    o.alpha = o.bad ? 0.0 : rho / pi;
+    o.rr = xs->rr[s];
+    const double nr = sqrt(o.rr);
+    o.due = nr < MIXED_DELTA * xs->mx[s] || xs->sigma[s] * nr < st->tol;
+    o.beta = rho > 0.0 ? o.rr / rho : 0.0;
+    return o;
+}
+
+/* r = fl32(r - alpha t), (r, r) into xs->rr[s]; the products of two floats are exact in fp64 */
+__global__ void __launch_bounds__(BLAS1_THREADS)
+mixed_update_r_kernel(int n, const acgb200_devstate *st, acgb200_xstate *xs, const float *__restrict__ t,
+                      float *__restrict__ r)
+{
+    __shared__ double red[BLAS1_THREADS / 32];
+    pdl_prologue();
+    const Gate g = gate_read(&st->ctrl[0], st);
+    if (!g.active) return;
+    const int s = g.iter & 1;
+    const double pi = xs->pi[s];
+    if (!(pi != 0.0 && isfinite(pi))) return;
+    const double alpha = xs->rho[s] / pi;
+    double acc = 0.0;
+    const int n2 = n >> 1;
+    const float2 *t2 = reinterpret_cast<const float2 *>(t);
+    float2 *r2 = reinterpret_cast<float2 *>(r);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n2; i += gridDim.x * blockDim.x) {
+        const float2 tv = t2[i];
+        float2 rv = r2[i];
+        rv.x = (float) __dsub_rn(rv.x, __dmul_rn(alpha, tv.x));
+        rv.y = (float) __dsub_rn(rv.y, __dmul_rn(alpha, tv.y));
+        r2[i] = rv;
+        acc = fma((double) rv.x, (double) rv.x, acc);
+        acc = fma((double) rv.y, (double) rv.y, acc);
+    }
+    if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0) {
+        const float rv = (float) __dsub_rn(r[n - 1], __dmul_rn(alpha, t[n - 1]));
+        r[n - 1] = rv;
+        acc = fma((double) rv, (double) rv, acc);
+    }
+    acc = block_sum(acc, red);
+    if (threadIdx.x == 0) atomicAdd(&xs->rr[s], acc);
+}
+
+__device__ __forceinline__ void mixed_yp_row(const MixedStep &k, double sigma, float ri, float &pi, float &yi, double &xi)
+{
+    const float yn = (float) __dadd_rn(yi, __dmul_rn(k.alpha, pi));
+    if (k.due) {
+        xi = __dadd_rn(xi, sigma * (double) yn);          /* sigma is a power of two: the product is exact */
+        yi = 0.0f;
+    } else {
+        yi = yn;
+        pi = (float) __dadd_rn(ri, __dmul_rn(k.beta, pi));
+    }
+}
+
+/* y = fl32(y + alpha p); not due: p = fl32(r + beta p); due: x += sigma y (fp64), y = 0 and p is left for
+ * the replacement.  Block 0 writes ctrl[1] (iteration k+1, or done on a breakdown) and ctrl[2] (active,
+ * iteration k, only when a reliable update is due), the next slot when none is due, and zeroes the next
+ * accumulators (and rr64[s] for this iteration's fp64 residual). */
+__global__ void __launch_bounds__(BLAS1_THREADS)
+mixed_update_yp_kernel(int n, acgb200_devstate *st, acgb200_xstate *xs, const float *__restrict__ r,
+                       float *__restrict__ p, float *__restrict__ y, double *__restrict__ x)
+{
+    pdl_prologue();
+    const Gate g = gate_read(&st->ctrl[0], st);
+    const int s = g.iter & 1;
+    const MixedStep k = mixed_step(st, xs, s);
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        acgb200_ctrl c1 = st->ctrl[0], c2 = st->ctrl[0];
+        c2.done = 1;
+        if (g.active) {
+            if (k.bad) { c1.done = 1; xs->breakdown = 1; }
+            else {
+                c1.iter = g.iter + 1;
+                if (k.due) { c2.done = 0; xs->rr64[s] = 0.0; }
+                else {
+                    xs->rho[s ^ 1] = k.rr; xs->mx[s ^ 1] = fmax(xs->mx[s], sqrt(k.rr)); xs->sigma[s ^ 1] = xs->sigma[s];
+                }
+            }
+            xs->pi[s ^ 1] = 0.0;
+            xs->rr[s ^ 1] = 0.0;
+        }
+        st->ctrl[1] = c1;
+        st->ctrl[2] = c2;
+    }
+    if (!g.active || k.bad) return;
+    const double sigma = xs->sigma[s];
+    const int n2 = n >> 1;
+    const float2 *r2 = reinterpret_cast<const float2 *>(r);
+    float2 *p2 = reinterpret_cast<float2 *>(p);
+    float2 *y2 = reinterpret_cast<float2 *>(y);
+    double2 *x2 = reinterpret_cast<double2 *>(x);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n2; i += gridDim.x * blockDim.x) {
+        const float2 rv = k.due ? make_float2(0.0f, 0.0f) : r2[i];
+        float2 pv = p2[i], yv = y2[i];
+        double2 xv = k.due ? x2[i] : make_double2(0.0, 0.0);
+        mixed_yp_row(k, sigma, rv.x, pv.x, yv.x, xv.x);
+        mixed_yp_row(k, sigma, rv.y, pv.y, yv.y, xv.y);
+        y2[i] = yv;
+        if (k.due) x2[i] = xv;
+        else p2[i] = pv;
+    }
+    if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0) {
+        float pv = p[n - 1], yv = y[n - 1];
+        double xv = x[n - 1];
+        mixed_yp_row(k, sigma, r[n - 1], pv, yv, xv);
+        y[n - 1] = yv;
+        if (k.due) x[n - 1] = xv;
+        else p[n - 1] = pv;
+    }
+}
+
+/* sigma' = 2^round(log2 sqrt(rr64)) as its exponent */
+__device__ __forceinline__ int mixed_scale_exp(double rr64)
+{
+    int e = 0;
+    const double m = frexp(sqrt(rr64), &e);
+    return m < 0.70710678118654752440 ? e - 1 : e;
+}
+
+/* The reliable update's second half (gated by ctrl[2]): r64 = b - A x has just been formed with
+ * rr64 = (r64, r64).  sqrt(rr64) < tol, or rr64 = 0, ends the solve (the iteration counted); otherwise
+ * sigma' = 2^round(log2 sqrt(rr64)), p = fl32(r64/sigma' + beta (sigma/sigma') p) with
+ * beta = (rr64/sigma^2)/rho_k, r = fl32(r64/sigma'), and the next slot restarts M.  Block 0 writes ctrl[0]:
+ * the word above, or ctrl[1] when no update was due. */
+__global__ void __launch_bounds__(BLAS1_THREADS)
+mixed_replace_kernel(int n, acgb200_devstate *st, acgb200_xstate *xs, const double *__restrict__ r64,
+                     float *__restrict__ r, float *__restrict__ p)
+{
+    pdl_prologue();
+    const Gate g = gate_read(&st->ctrl[2], st);
+    const int s = g.iter & 1;
+    const double rr64 = xs->rr64[s];
+    const bool stop = sqrt(rr64) < st->tol || rr64 == 0.0;
+    const int e = g.active && !stop ? mixed_scale_exp(rr64) : 0;
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        acgb200_ctrl c = st->ctrl[1];
+        if (g.active) {
+            xs->nupdates += 1;
+            xs->last_rr64 = rr64;
+            c.iter = g.iter + 1; c.done = 0;
+            if (stop) { c.done = 1; xs->conv = 1; }
+            else {
+                const double rho = ldexp(rr64, -2 * e);
+                xs->rho[s ^ 1] = rho; xs->mx[s ^ 1] = sqrt(rho); xs->sigma[s ^ 1] = ldexp(1.0, e);
+            }
+        }
+        st->ctrl[0] = c;
+    }
+    if (!g.active || stop) return;
+    const double sigma = xs->sigma[s];
+    const double is = ldexp(1.0, -e);
+    const double bf = (rr64 / (sigma * sigma)) / xs->rho[s] * (sigma * is);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const double rv = r64[i] * is;
+        p[i] = (float) __dadd_rn(rv, __dmul_rn(bf, (double) p[i]));
+        r[i] = (float) rv;
+    }
+}
+
+/* x += sigma y */
+__global__ void __launch_bounds__(BLAS1_THREADS)
+mixed_fold_kernel(int n, double sigma, const float *__restrict__ y, double *__restrict__ x)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        x[i] = __dadd_rn(x[i], sigma * (double) y[i]);
+}
+
 /* ------------------------------------------------------------------------ */
 /* host-side launchers (C linkage)                                           */
 /* ------------------------------------------------------------------------ */
@@ -2501,6 +2748,18 @@ static symdiag_fn symdiag_variant(int UB, int T, bool pcg, bool coded)
 static symdiag_fn symdiag_variant(const acgb200_spmvplan *pl, bool pcg)
 {
     return symdiag_variant(pl->slice_ub, pl->slice_threads, pcg, pl->symdiag_codes > 0);
+}
+
+/* the float-vector product of the mixed-precision solve, for the same (UB, T) pairs */
+static symdiag_fn symdiag_f32_variant(const acgb200_spmvplan *pl)
+{
+    const int UB = pl->slice_ub, T = pl->slice_threads;
+    const bool coded = pl->symdiag_codes > 0;
+#define X(u, t) if (UB == u && T == t) \
+        return coded ? spmv_symdiag_kernel<u, t, false, uint8_t, float> : spmv_symdiag_kernel<u, t, false, double, float>;
+    X(5, 128) X(7, 128) X(8, 128) X(9, 128) X(7, 256) X(8, 256) X(9, 256)
+#undef X
+    return NULL;
 }
 
 /* the kernel's view of the plan's stored diagonals, fp64 or coded */
@@ -3008,6 +3267,82 @@ extern "C" int acgb200_minres_update(int n, acgb200_devstate *st, acgb200_nstate
     static int occ = 0;
     return (int) launch_chain(minres_update_kernel, blas1_grid(n, (const void *) minres_update_kernel, &occ),
                               BLAS1_THREADS, 0, stream, n, st, ns, cin, cout, v, u, w, wprev, x, vnext);
+}
+
+extern "C" int acgb200_spmv_f32_launch(const acgb200_spmvf32args *a, cudaStream_t stream)
+{
+    const acgb200_spmvplan *pl = a->plan;
+    if (pl->nslices > 0 && pl->symdiag_nd > 0) {
+        const symdiag_fn fn = symdiag_f32_variant(pl);
+        if (!fn) return (int) cudaErrorInvalidConfiguration;
+        int per_sm = 0;
+        const cudaError_t oe = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void *) fn, pl->slice_threads, 0);
+        if (oe) return (int) oe;
+        SymdiagParams S;
+        memset(&S, 0, sizeof(S));
+        symdiag_params(pl, S);
+        S.x = reinterpret_cast<const double *>(a->x); S.y = reinterpret_cast<double *>(a->y);
+        S.acc = a->acc; S.dotrows = pl->nrows;
+        S.mode = a->acc ? SPMV_Y_AX_DOT : SPMV_Y_AX;
+        S.ctrl_in = a->ctrl_in; S.st = (acgb200_devstate *) a->st;
+        /* the fp64 product's grid (its L2 cap included), unless the float instantiation fits fewer CTAs */
+        const long long fgrid = (long long) acgb200_num_sms() * (per_sm < 1 ? 1 : per_sm);
+        const int grid = (int) (fgrid < pl->slice_grid ? fgrid : pl->slice_grid);
+        const cudaError_t le = launch_chain(fn, grid, pl->slice_threads, (size_t) 0, stream, S);
+        if (le) return (int) le;
+    }
+    if (a->nranges > 0) {
+        static int occ = 0;
+        if (occ == 0 && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (const void *) spmv_rows_f32_kernel, MIXED_ROWS_T, 0) || occ < 1))
+            occ = 1;
+        long long grid = (long long) acgb200_num_sms() * occ;
+        const long long need = ((long long) a->nranges + MIXED_ROWS_T / 32 - 1) / (MIXED_ROWS_T / 32);
+        if (grid > need) grid = need;
+        const cudaError_t le = launch_chain(spmv_rows_f32_kernel, (int) (grid < 1 ? 1 : grid), MIXED_ROWS_T, (size_t) 0,
+                                            stream, a->nranges, reinterpret_cast<const int2 *>(a->ranges), a->rowptr,
+                                            a->colidx, a->a, a->x, a->y, a->acc, a->ctrl_in, a->st);
+        if (le) return (int) le;
+    }
+    return (int) cudaGetLastError();
+}
+
+extern "C" int acgb200_mixed_setup(int n, double scale, const double *r64, float *r, float *p, float *y, cudaStream_t stream)
+{
+    static int occ = 0;
+    mixed_setup_kernel<<<blas1_grid(n, (const void *) mixed_setup_kernel, &occ), BLAS1_THREADS, 0, stream>>>(
+        n, scale, r64, r, p, y);
+    return (int) cudaGetLastError();
+}
+
+extern "C" int acgb200_mixed_update_r(int n, const acgb200_devstate *st, acgb200_xstate *xs, const float *t, float *r,
+                                      cudaStream_t stream)
+{
+    static int occ = 0;
+    return (int) launch_chain(mixed_update_r_kernel, blas1_grid(n, (const void *) mixed_update_r_kernel, &occ),
+                              BLAS1_THREADS, 0, stream, n, st, xs, t, r);
+}
+
+extern "C" int acgb200_mixed_update_yp(int n, acgb200_devstate *st, acgb200_xstate *xs, const float *r, float *p,
+                                       float *y, double *x, cudaStream_t stream)
+{
+    static int occ = 0;
+    return (int) launch_chain(mixed_update_yp_kernel, blas1_grid(n, (const void *) mixed_update_yp_kernel, &occ),
+                              BLAS1_THREADS, 0, stream, n, st, xs, r, p, y, x);
+}
+
+extern "C" int acgb200_mixed_replace(int n, acgb200_devstate *st, acgb200_xstate *xs, const double *r64, float *r,
+                                     float *p, cudaStream_t stream)
+{
+    static int occ = 0;
+    return (int) launch_chain(mixed_replace_kernel, blas1_grid(n, (const void *) mixed_replace_kernel, &occ),
+                              BLAS1_THREADS, 0, stream, n, st, xs, r64, r, p);
+}
+
+extern "C" int acgb200_mixed_fold(int n, double sigma, const float *y, double *x, cudaStream_t stream)
+{
+    static int occ = 0;
+    mixed_fold_kernel<<<blas1_grid(n, (const void *) mixed_fold_kernel, &occ), BLAS1_THREADS, 0, stream>>>(n, sigma, y, x);
+    return (int) cudaGetLastError();
 }
 
 extern "C" int acgb200_gather(int n, double *dst, const double *src, const int *idx, cudaStream_t stream)

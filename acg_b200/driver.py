@@ -24,7 +24,7 @@ import numpy as np
 
 SOLVERS = {"acg": "solvempi", "acg-pipelined": "solve_pipelined",
            "acg-device": "solve_device", "acg-device-pipelined": "solve_device_pipelined",
-           "minres": "solve_minres"}
+           "minres": "solve_minres", "mixed": "solve_mixed"}
 
 
 def parse_args(argv=None):
@@ -33,7 +33,8 @@ def parse_args(argv=None):
     ap.add_argument("--binary", action="store_true", help="aCG binary encoding (mtx2bin); required for more than one process")
     ap.add_argument("--solver", default="acg", choices=sorted(SOLVERS),
                     help="minres: MINRES for symmetric indefinite or singular A, e.g. with a negative --epsilon "
-                         "(acgsolvercuda_solve_minres; one process only)")
+                         "(acgsolvercuda_solve_minres; one process only); mixed: CG with float vectors and "
+                         "reliable updates to an fp64 tolerance (acgsolvercuda_solve_mixed; one process only)")
     ap.add_argument("--max-iterations", type=int, default=100)
     ap.add_argument("--residual-atol", type=float, default=0.0)
     ap.add_argument("--residual-rtol", type=float, default=1e-9)
@@ -175,22 +176,24 @@ def solve_shifted(args, A, cg, log):
 
 
 def solve_minres(args, A, cg, log):
-    """The --solver minres run: one solve_minres call, the solver report, then the iterations, MINRES's
-    recursively updated residual norm and the true residual ||b - A x|| (and the error norms with
+    """The --solver minres and --solver mixed runs: one solve_minres or solve_mixed call, the solver report,
+    then the iterations (and reliable updates), the solver's residual norm -- MINRES's recursively updated
+    one, the mixed solve's fp64 one -- and the true residual ||b - A x|| (and the error norms with
     --manufactured-solution)."""
     n = A.c.nownedrows
     bo, xstar = local_rhs(args, A, n)
     b = A.vector(); x = A.vector()
     b.x[:] = 0.0
     b.x[:n] = bo
-    code = cg.solve_minres(b, x, maxits=args.max_iterations, residualatol=args.residual_atol,
-                           residualrtol=args.residual_rtol, warmup=args.warmup)
+    code = getattr(cg, SOLVERS[args.solver])(b, x, maxits=args.max_iterations, residualatol=args.residual_atol,
+                                             residualrtol=args.residual_rtol, warmup=args.warmup)
     log(cg.report())
     import scipy.sparse as sp
     rp = A.frowptr[:n + 1]
     F = sp.csr_matrix((A.fa[:rp[n]], A.fcolidx[:rp[n]] - A.c.rowidxbase, rp), shape=(n, n))
     true = float(np.linalg.norm(bo - F @ x.x[:n]))
-    log(f"minres: iterations {cg.c.niterations} residual 2-norm {cg.c.rnrm2:.15g} "
+    upd = f" reliable updates {cg.info()['mixed_reliable_updates']}" if args.solver == "mixed" else ""
+    log(f"{args.solver}: iterations {cg.c.niterations}{upd} residual 2-norm {cg.c.rnrm2:.15g} "
         f"true residual 2-norm {true:.15g} relative {true / cg.c.bnrm2 if cg.c.bnrm2 else 0.0:.3e}")
     if xstar is not None:
         log(f"initial error 2-norm: {np.linalg.norm(xstar):.15g}")
@@ -215,11 +218,12 @@ def main(argv=None):
     from . import dist as abdist, mtxio
     from .api import SolverCuda, SymCsrMatrix, mtx_info
 
-    if args.solver == "minres":
+    if args.solver in ("minres", "mixed"):
         if int(os.environ.get("WORLD_SIZE", "1")) > 1:
-            raise SystemExit("--solver minres runs in one process (one GPU, the whole matrix)")
+            raise SystemExit(f"--solver {args.solver} runs in one process (one GPU, the whole matrix)")
         if args.nrhs is not None or args.shifts is not None:
-            raise SystemExit("--solver minres cannot be combined with --nrhs or --shifts (one system, classic CG options)")
+            raise SystemExit(f"--solver {args.solver} cannot be combined with --nrhs or --shifts "
+                             "(one system, classic CG options)")
     if args.nrhs is not None:
         if not 1 <= args.nrhs <= 8:
             raise SystemExit("--nrhs must be between 1 and 8")
@@ -288,7 +292,7 @@ def main(argv=None):
         cg.free()
         comm.destroy()
         return 0 if code == 0 else 1
-    if args.solver == "minres":
+    if args.solver in ("minres", "mixed"):
         code = solve_minres(args, A, cg, log)
         cg.free()
         comm.destroy()

@@ -122,6 +122,29 @@ ACG_API int acgsolvercuda_solve_minres(struct acgsolvercuda *cg, const struct ac
                                        const struct acgvector *b, struct acgvector *x, int maxits,
                                        double residualatol, double residualrtol, int warmup, int *errcode);
 
+/* A x = b for symmetric positive definite A to an fp64 tolerance with float vectors: CG whose r, p, A p and
+ * solution increment y are stored in fp32 (every operation in fp64, each stored value rounded once, scaled
+ * by a power of two), with reliable updates (Sleijpen & van der Vorst, Computing 56, 1996; van der Vorst &
+ * Ye, SISC 22, 2000): when the fp32 residual has fallen by 0.1 since the last update, or when it meets the
+ * tolerance, y is folded into the fp64 x and r is replaced by b - A x from the fp64 product.  Arguments as
+ * acgsolvercuda_solve_minres.  tol = threshold(atol, rtol, ||r0||); convergence is only declared on the
+ * fp64 residual ||b - A x|| (strict <) of the x returned, and rnrm2 is always that figure, also when the
+ * solve stops at maxits (the increment is folded in and the residual recomputed).  ACG_ERR_NOT_CONVERGED
+ * follows acgsolvercuda_solvempi's rule.  maxits = 0 returns x0 unchanged; ||r0|| < tol or ||r0|| = 0
+ * runs no iteration.  (p, A p) = 0 or non-finite ends the solve before that iteration's update, which is
+ * not counted; x is then the last fold.  niterations counts CG steps (fp32 products);
+ * acgb200_info.mixed_reliable_updates the reliable updates.  One GPU, unpartitioned matrix: ghost rows or
+ * more than one rank give ACG_ERR_NOT_SUPPORTED.  `warmup` iterations run first on scratch state; the
+ * results do not depend on them. */
+ACG_API int acgsolvercuda_solve_mixed(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A,
+                                      const struct acgvector *b, struct acgvector *x, int maxits,
+                                      double residualatol, double residualrtol, int warmup, int *errcode);
+
+/* The fp32 product of acgsolvercuda_solve_mixed on host float vectors over the owned rows: y = fl32(A x),
+ * each row's sum formed in fp64 from the widened x, and *dot (may be NULL) = sum x_i y_i in fp64.  y is
+ * poisoned on the device first.  One GPU, unpartitioned matrix.  For tests of the fp32 product. */
+ACG_API int acgsolvercuda_spmv_f32(struct acgsolvercuda *cg, const float *x, float *y, double *dot);
+
 struct acgb200_info {
     int spmv_lanes_per_row, spmv_rows_cap, spmv_nnz_cap, spmv_stages;
     int spmv_ntiles, spmv_nlong, spmv_grid, spmv_smem_bytes;
@@ -162,6 +185,7 @@ struct acgb200_info {
     int spmv_symdiag_codes;                     /* entries of the value table when the stored diagonals are one-byte
                                                    codes into it (option "symdiag_codes"); 0: fp64 diagonals */
     int64_t spmv_symdiag_code_bytes;            /* the codes' bytes, one per element of the diagonals; 0: no codes */
+    int mixed_reliable_updates;                 /* reliable updates of the last acgsolvercuda_solve_mixed */
 };
 ACG_API int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info);
 
