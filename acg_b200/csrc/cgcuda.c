@@ -154,6 +154,9 @@ int acgb200_set_option(const char *key, int value)
 
 struct evpool { cudaEvent_t *ev; int n, cap; };
 
+/* the loops a solver runs; each has its own cached graph */
+enum solve_kind { KIND_CLASSIC, KIND_PIPELINED, KIND_MULTI, KIND_SHIFTED, KIND_MINRES, KIND_MIXED, NKINDS };
+
 struct priv {
     const struct acgsolvercuda *key;
     const void *d_r_id;                 /* cg->d_r: identifies the solver if the caller moves the struct */
@@ -171,11 +174,9 @@ struct priv {
     struct acgcomm redcomm;             /* private duplicate of the caller's communicator for reductions */
     int have_redcomm;
     double *d_b, *d_x;                  /* right-hand side / solution on the device, kept between solves */
-    cudaGraphExec_t graph[6];           /* [0] classic, [1] pipelined, [2] several right-hand sides, [3] shifted
-                                         * systems, [4] MINRES, [5] mixed precision: two iterations each (parity 0
-                                         * then 1) */
-    int graph_sig[6];                   /* loop configuration each cached graph was captured with (graph_signature) */
-    int graph_launches[6];              /* kernel/NCCL launches inside one replay */
+    cudaGraphExec_t graph[NKINDS];      /* per solve kind: two iterations (parity 0 then 1) */
+    int graph_sig[NKINDS];              /* loop configuration each cached graph was captured with (graph_signature) */
+    int graph_launches[NKINDS];         /* kernel/NCCL launches inside one replay */
     double last_h2d_ms, last_d2h_ms;    /* host time spent before / after the solve window */
     cudaEvent_t ev_t0, ev_t1;           /* device-side bracket of the solve window */
     double last_solve_ms;
@@ -295,7 +296,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
             pv->p2p.window = NULL;
         }
         if (pv->have_redcomm && pv->redcomm.ncclcomm) ncclCommDestroy(pv->redcomm.ncclcomm);
-        for (int i = 0; i < 6; i++) if (pv->graph[i]) cudaGraphExecDestroy(pv->graph[i]);
+        for (int i = 0; i < NKINDS; i++) if (pv->graph[i]) cudaGraphExecDestroy(pv->graph[i]);
         cudaFree(pv->plan.d_tiles); cudaFree(pv->plan.d_longrows); cudaFree(pv->plan.d_long_scratch); cudaFree(pv->plan.d_medrows);
         cudaFree(pv->plan.d_slices); cudaFree(pv->plan.d_sval); cudaFree(pv->plan.d_spatoff); cudaFree(pv->plan.d_spatid);
         cudaFree(pv->plan.d_hval); cudaFree(pv->plan.d_symdiag_bad); cudaFree(pv->plan.d_hcode); cudaFree(pv->plan.d_codes);
@@ -897,12 +898,11 @@ struct solvectx {
     int capturing;            /* inside cudaStreamBeginCapture: no profiling marks */
     int p2p;                  /* loop exchanges go through peer memory */
     int mk;                   /* multi-vector loop: block width K (0: single vector) */
-    int shifted;              /* shifted-systems loop (acgsolvercuda_solve_shifted) */
-    int minres;               /* MINRES loop (acgsolvercuda_solve_minres) */
-    int mixed;                /* mixed-precision loop (acgsolvercuda_solve_mixed) */
+    enum solve_kind kind;     /* the loop iterate() runs, and so its graph slot */
     int fused;                /* pipelined loop: one fused iteration (acgb200_pcg_fused_launch); its control word
                                * alternates between ctrl[0] and ctrl[1] by iteration parity */
     int issued;               /* iterations iterate() issued, inactive ones included */
+    double t0;                /* host clock at the start of the solve window */
 };
 
 static int evpool_reserve(struct evpool *p, int n)
@@ -930,6 +930,61 @@ static double evpool_sum_ms(struct evpool *p)
         if (cudaEventElapsedTime(&ms, p->ev[i], p->ev[i + 1]) == cudaSuccess) tot += ms;
     }
     return tot;
+}
+
+/* Open the timed window of a solve: profile events for up to maxits + 3 products, the counters of the last
+ * solve reset, every rank past the barrier and the stream idle before the clocks start. */
+static int window_open(struct solvectx *c, int maxits, double atol, double rtol, double diffatol, double diffrtol)
+{
+    struct acgsolvercuda *cg = c->cg;
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    if (cfg.profile) {
+        OK(evpool_reserve(&pv->gemv, 2 * (maxits + 3)));
+        OK(evpool_reserve(&pv->blas, 2 * (maxits + 3)));
+    }
+    pv->gemv.n = pv->blas.n = 0;
+    cg->nsolves++; cg->niterations = 0;
+    cg->bnrm2 = cg->r0nrm2 = cg->rnrm2 = cg->x0nrm2 = cg->dxnrm2 = INFINITY;
+    cg->maxits = maxits; cg->diffatol = diffatol; cg->diffrtol = diffrtol;
+    cg->residualatol = atol; cg->residualrtol = rtol;
+    /* what acgsolvercuda_info reports of the last solve, whichever entry point runs it */
+    pv->last_fused = c->fused;
+    pv->last_mixed_updates = 0;
+    pv->last_spmv_ms = pv->last_blas_ms = 0; pv->last_spmv_n = 0;
+    OK(acgcomm_barrier(pv->stream, c->comm, errcode));
+    CU(cudaStreamSynchronize(pv->stream));
+    c->t0 = wall();
+    CU(cudaEventRecord(pv->ev_t0, pv->stream));
+    c->launches = 0;
+    return ACG_SUCCESS;
+}
+
+/* Close it: solve time on the host and device clocks, launches, and the profiled product and update times */
+static int window_close(struct solvectx *c)
+{
+    struct acgsolvercuda *cg = c->cg;
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    CU(cudaEventRecord(pv->ev_t1, pv->stream));
+    CU(cudaEventSynchronize(pv->ev_t1));
+    cg->tsolve += wall() - c->t0;
+    { float ms = 0; if (cudaEventElapsedTime(&ms, pv->ev_t0, pv->ev_t1) == cudaSuccess) pv->last_solve_ms = ms; }
+    pv->last_launches = c->launches;
+    if (cfg.profile) {
+        pv->last_spmv_ms = evpool_sum_ms(&pv->gemv); pv->last_spmv_n = pv->gemv.n / 2;
+        pv->last_blas_ms = evpool_sum_ms(&pv->blas);
+        cg->tgemv += 1e-3 * pv->last_spmv_ms;
+        cg->taxpy += 1e-3 * pv->last_blas_ms;
+    }
+    return ACG_SUCCESS;
+}
+
+/* the return-code rule of acg/cgcuda.c:1099-1107: a solve that did not converge fails unless both
+ * tolerances are off */
+static int not_converged(int converged, double atol, double rtol_scaled)
+{
+    return !converged && !(atol == 0 && rtol_scaled == 0);
 }
 
 /* offdiag_kernel's share of the epilogue of `mode` (o->acc set): add the border x ghost block to
@@ -1043,6 +1098,21 @@ static int allreduce(struct solvectx *c, const double *src, double *dst, int cou
     return acgcomm_allreduce(src, dst, count, ACG_DOUBLE, ACG_SUM, c->pv->stream, c->comm, c->errcode);
 }
 
+/* the communicator of the one-GPU entry points */
+static struct acgcomm null_comm(void)
+{
+    struct acgcomm null;
+    memset(&null, 0, sizeof(null));
+    null.type = acgcomm_null;
+    return null;
+}
+
+/* one GPU, whole matrix: what the multi-vector, shifted, MINRES and mixed-precision paths support */
+static int one_gpu(const struct priv *pv, const struct acgsymcsrmatrix *A)
+{
+    return pv->nghost == 0 && pv->commsize == 1 && !(A && A->nghostrows > 0);
+}
+
 /* global sum of a device-side reduction result, brought to the host */
 static int reduce_to_host(struct solvectx *c, double *loc, double *glob, int count, double *host)
 {
@@ -1050,6 +1120,20 @@ static int reduce_to_host(struct solvectx *c, double *loc, double *glob, int cou
     OK(allreduce(c, loc, glob, count));
     CU(cudaMemcpyAsync(host, c->multi ? glob : loc, (size_t) count * sizeof(double), cudaMemcpyDeviceToHost, c->pv->stream));
     CU(cudaStreamSynchronize(c->pv->stream));
+    return ACG_SUCCESS;
+}
+
+/* x0 from the caller's vector to the device; the time goes to last_h2d_ms */
+static int upload_x0(struct solvectx *c, const struct acgvector *x)
+{
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    const double tb = wall();
+    /* a caller may hand over a longer vector than this part's owned + ghost entries: only those are used */
+    const size_t nx = (size_t) (x->num_nonzeros < pv->nvec ? x->num_nonzeros : pv->nvec);
+    CU(cudaMemcpyAsync(c->d_x, x->x, nx * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
+    CU(cudaStreamSynchronize(pv->stream));
+    pv->last_h2d_ms += 1e3 * (wall() - tb);
     return ACG_SUCCESS;
 }
 
@@ -1081,14 +1165,10 @@ static int solve_begin(struct solvectx *c, struct acgsolvercuda *cg, const struc
         CU(cudaMemsetAsync(pv->d_x, 0, vbytes, pv->stream));
     }
     c->d_b = pv->d_b; c->d_x = pv->d_x;
-    /* a caller may hand over longer vectors than this part's owned + ghost entries: only those are used */
     const size_t nb = (size_t) (b->num_nonzeros < pv->nvec ? b->num_nonzeros : pv->nvec);
-    const size_t nx = (size_t) (x->num_nonzeros < pv->nvec ? x->num_nonzeros : pv->nvec);
     CU(cudaMemcpyAsync(c->d_b, b->x, nb * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
-    CU(cudaMemcpyAsync(c->d_x, x->x, nx * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
-    CU(cudaStreamSynchronize(pv->stream));
     pv->last_h2d_ms = 1e3 * (wall() - tb);
-    return ACG_SUCCESS;
+    return upload_x0(c, x);
 }
 
 static int solve_end(struct solvectx *c, struct acgvector *x, int status)
@@ -1103,24 +1183,25 @@ static int solve_end(struct solvectx *c, struct acgvector *x, int status)
     return status;
 }
 
-static int push_state(struct solvectx *c, const struct acgb200_devstate *st)
+/* one struct of device scalars (d_st, d_ms, d_ss, d_ns, d_xs) from the host through its pinned staging buffer */
+static int scalars_push(struct solvectx *c, void *dev, void *pinned, const void *src, size_t bytes)
 {
     int *errcode = c->errcode;
     /* everything queued before must be done with the staging buffer and with
      * the device state it is about to replace */
     CU(cudaStreamSynchronize(c->pv->stream));
-    *c->pv->h_st = *st;
-    CU(cudaMemcpyAsync(c->pv->d_st, c->pv->h_st, sizeof(*st), cudaMemcpyHostToDevice, c->pv->stream));
+    memcpy(pinned, src, bytes);
+    CU(cudaMemcpyAsync(dev, pinned, bytes, cudaMemcpyHostToDevice, c->pv->stream));
     CU(cudaStreamSynchronize(c->pv->stream));
     return ACG_SUCCESS;
 }
 
-static int pull_state(struct solvectx *c, struct acgb200_devstate *st)
+static int scalars_pull(struct solvectx *c, const void *dev, void *pinned, void *dst, size_t bytes)
 {
     int *errcode = c->errcode;
-    CU(cudaMemcpyAsync(c->pv->h_st, c->pv->d_st, sizeof(*st), cudaMemcpyDeviceToHost, c->pv->stream));
+    CU(cudaMemcpyAsync(pinned, dev, bytes, cudaMemcpyDeviceToHost, c->pv->stream));
     CU(cudaStreamSynchronize(c->pv->stream));
-    *st = *c->pv->h_st;
+    memcpy(dst, pinned, bytes);
     return ACG_SUCCESS;
 }
 
@@ -1138,20 +1219,20 @@ static double threshold(double atol, double rtol, double r0nrm2)
  * pointers the kernels and NCCL calls use are fixed for the life of the solver
  * and the iteration index only enters through its parity, so one two-iteration
  * graph serves the whole solve (and later solves). */
-/* everything besides the (fixed) pointers that decides which kernels and NCCL calls an iteration issues:
- * a cached graph is only replayed for the configuration it was captured with (options can change between
- * two solves on one solver) */
+/* everything besides the (fixed) pointers and the solve kind (its own slot) that decides which kernels and
+ * NCCL calls an iteration issues: a cached graph is only replayed for the configuration it was captured with
+ * (options can change between two solves on one solver) */
 static int graph_signature(const struct solvectx *c)
 {
     return 1 | (c->multi ? 2 : 0) | (c->p2p ? 4 : 0) | (c->pv->p2p.h_desc.fuse ? 8 : 0) | (cfg.pdl ? 16 : 0)
-           | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0) | (c->shifted ? 128 : 0) | (c->mk << 8)
-           | (c->fused ? 1 << 16 : 0) | (c->minres ? 1 << 17 : 0) | (c->mixed ? 1 << 18 : 0);
+           | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0) | (c->mk << 8) | (c->fused ? 1 << 16 : 0);
 }
 
-static int capture_pair(struct solvectx *c, int kind, int (*issue)(struct solvectx *, int))
+static int capture_pair(struct solvectx *c, int (*issue)(struct solvectx *, int))
 {
     struct priv *pv = c->pv;
     int *errcode = c->errcode;
+    const enum solve_kind kind = c->kind;
     if (pv->graph[kind] && pv->graph_sig[kind] == graph_signature(c)) return ACG_SUCCESS;
     if (pv->graph[kind]) { cudaGraphExecDestroy(pv->graph[kind]); pv->graph[kind] = NULL; }
     const int before = c->launches;
@@ -1176,10 +1257,11 @@ static int capture_pair(struct solvectx *c, int kind, int (*issue)(struct solvec
 /* Run `issue(c,k)` for k < maxits, polling the device control word.  The
  * first two iterations are issued directly (they also serve as the un-captured
  * first use of every NCCL path), the rest as replays of the two-iteration graph. */
-static int iterate(struct solvectx *c, int maxits, int poll, int kind, int (*issue)(struct solvectx *, int))
+static int iterate(struct solvectx *c, int maxits, int poll, int (*issue)(struct solvectx *, int))
 {
     struct priv *pv = c->pv;
     int *errcode = c->errcode;
+    const enum solve_kind kind = c->kind;
     int issued = 0, slot = 0, have_prev = 0, since_poll = 0;
     /* Replays are used on one GPU and with the peer-memory exchange (kernel nodes
      * only).  With the NCCL exchange the iteration also contains collectives on
@@ -1189,7 +1271,7 @@ static int iterate(struct solvectx *c, int maxits, int poll, int kind, int (*iss
     const int use_graph = cfg.graph && !cfg.profile && maxits >= 6 && (!c->multi || c->p2p || cfg.graph >= 2);
     while (issued < maxits) {
         if (use_graph && issued >= 2 && maxits - issued >= 2) {
-            if (!pv->graph[kind] || pv->graph_sig[kind] != graph_signature(c)) OK(capture_pair(c, kind, issue));
+            if (!pv->graph[kind] || pv->graph_sig[kind] != graph_signature(c)) OK(capture_pair(c, issue));
             CU(cudaGraphLaunch(pv->graph[kind], pv->stream));
             c->launches += pv->graph_launches[kind];
             issued += 2; since_poll += 2;
@@ -1286,8 +1368,8 @@ int acgsolvercuda_solvempi(
     const int n = pv->nowned;
     struct acgb200_devstate h;
 
+    c.kind = KIND_CLASSIC;
     c.p2p = c.multi && pv->p2p.enabled && cfg.p2p;
-    pv->last_fused = 0;
     /* a rank that is ahead must not store into a peer's window while that peer's kernels of the
      * previous solve are still reading it: order the first post of this solve behind every rank */
     if (c.p2p) OK(acgcomm_barrier(pv->stream, comm, errcode));
@@ -1298,7 +1380,7 @@ int acgsolvercuda_solvempi(
     if (warmup > 0) {
         memset(&h, 0, sizeof(h));
         h.maxits = warmup; h.rr_loc[0] = h.rr[0] = 1.0;
-        OK(push_state(&c, &h));
+        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
         double *xsave = c.d_x; c.d_x = cg->d_r;
         if (c.p2p) {
             OK(acgb200_p2p_begin(&pv->p2p, warmup, pv->stream));
@@ -1309,25 +1391,11 @@ int acgsolvercuda_solvempi(
         KL(acgb200_dot(n, c.d_b, c.d_b, &st->tmp_loc[0], pv->stream));
         CU(cudaStreamSynchronize(pv->stream));
     }
-    if (cfg.profile) {
-        OK(evpool_reserve(&pv->gemv, 2 * (maxits + 2)));
-        OK(evpool_reserve(&pv->blas, 2 * (maxits + 2)));
-    }
-    pv->gemv.n = pv->blas.n = 0;
-
-    cg->nsolves++; cg->niterations = 0;
-    cg->bnrm2 = cg->r0nrm2 = cg->rnrm2 = cg->x0nrm2 = cg->dxnrm2 = INFINITY;
-    cg->maxits = maxits; cg->diffatol = diffatol; cg->diffrtol = diffrtol;
-    cg->residualatol = residualatol; cg->residualrtol = residualrtol;
-    OK(acgcomm_barrier(pv->stream, comm, errcode));
-    CU(cudaStreamSynchronize(pv->stream));
-    const double t0 = wall();
-    CU(cudaEventRecord(pv->ev_t0, pv->stream));
-    c.launches = 0;
+    OK(window_open(&c, maxits, residualatol, residualrtol, diffatol, diffrtol));
 
     /* ||b|| (acg/cgcuda.c:727-739) */
     memset(&h, 0, sizeof(h));
-    OK(push_state(&c, &h));
+    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
     double bb = 0, rr0 = 0;
     KL(acgb200_dot(n, c.d_b, c.d_b, &st->tmp_loc[0], pv->stream));
     OK(reduce_to_host(&c, &st->tmp_loc[0], &st->tmp[0], 1, &bb));
@@ -1348,14 +1416,14 @@ int acgsolvercuda_solvempi(
         memset(&h, 0, sizeof(h));
         h.maxits = maxits; h.tol = tol;
         h.rr_loc[0] = h.rr[0] = rr0;
-        OK(push_state(&c, &h));
+        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
         if (c.p2p) {
             /* p_0 = r_0 goes to the neighbours' windows as exchange number 0 */
             OK(acgb200_p2p_begin(&pv->p2p, maxits, pv->stream));
             OK(post(&c, 0, 0, pvec, -1, NULL, 0, 0, 0, 0));
         }
-        OK(iterate(&c, maxits, tol > 0, 0, classic_iteration));
-        OK(pull_state(&c, &h));
+        OK(iterate(&c, maxits, tol > 0, classic_iteration));
+        OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
         cg->niterations = h.ctrl[0].iter;
         converged = h.ctrl[0].done;
         const double rr = converged ? h.final_rr
@@ -1363,22 +1431,9 @@ int acgsolvercuda_solvempi(
         cg->rnrm2 = sqrt(rr);
         cg->ntotaliterations += cg->niterations;
     }
-    CU(cudaEventRecord(pv->ev_t1, pv->stream));
-    CU(cudaEventSynchronize(pv->ev_t1));
-    const double t1 = wall();
-    cg->tsolve += t1 - t0;
-    { float ms = 0; if (cudaEventElapsedTime(&ms, pv->ev_t0, pv->ev_t1) == cudaSuccess) pv->last_solve_ms = ms; }
+    OK(window_close(&c));
     account_classic(cg, pv, cg->niterations, c.multi);
-    pv->last_launches = c.launches;
-    if (cfg.profile) {
-        pv->last_spmv_ms = evpool_sum_ms(&pv->gemv); pv->last_spmv_n = pv->gemv.n / 2;
-        pv->last_blas_ms = evpool_sum_ms(&pv->blas);
-        cg->tgemv += 1e-3 * pv->last_spmv_ms;
-        cg->taxpy += 1e-3 * pv->last_blas_ms;
-    }
-    int status = ACG_SUCCESS;
-    if (!converged && !(residualatol == 0 && rtol_scaled == 0)) status = ACG_ERR_NOT_CONVERGED;   /* :1099-1107 */
-    return solve_end(&c, x, status);
+    return solve_end(&c, x, not_converged(converged, residualatol, rtol_scaled) ? ACG_ERR_NOT_CONVERGED : ACG_SUCCESS);
 }
 
 int acgsolvercuda_solve(
@@ -1386,9 +1441,7 @@ int acgsolvercuda_solve(
     const struct acgvector *b, struct acgvector *x,
     int maxits, double diffatol, double diffrtol, double residualatol, double residualrtol, int warmup)
 {
-    struct acgcomm null;
-    memset(&null, 0, sizeof(null));
-    null.type = acgcomm_null;
+    struct acgcomm null = null_comm();
     int errcode = 0;
     return acgsolvercuda_solvempi(cg, A, b, x, maxits, diffatol, diffrtol, residualatol, residualrtol,
                                   warmup, &null, 0, &errcode, NULL, NULL, 0);
@@ -1467,7 +1520,9 @@ static int ensure_blocks(struct priv *pv, const struct acgsolvercuda *cg, int k,
     if (pv->mk >= k) return ACG_SUCCESS;
     double **blk[5] = { &pv->d_mx, &pv->d_mb, &pv->d_mr, &pv->d_mp, &pv->d_mt };
     for (int i = 0; i < 5; i++) { cudaFree(*blk[i]); *blk[i] = NULL; }
-    for (int i = 2; i < 4; i++) if (pv->graph[i]) { cudaGraphExecDestroy(pv->graph[i]); pv->graph[i] = NULL; }
+    const enum solve_kind blockloops[2] = { KIND_MULTI, KIND_SHIFTED };
+    for (int i = 0; i < 2; i++)
+        if (pv->graph[blockloops[i]]) { cudaGraphExecDestroy(pv->graph[blockloops[i]]); pv->graph[blockloops[i]] = NULL; }
     pv->mk = 0;
     /* one spare row: the BLAS-1 kernels read pairs of entries */
     const size_t bytes = ((size_t) pv->nowned + 1) * (size_t) k * sizeof(double);
@@ -1513,25 +1568,6 @@ static int download_block_vec(struct priv *pv, double *dst, const double *src, i
     if (!e) for (size_t i = 0; i < n; i++) memcpy(dst + i * (size_t) nrhs, tmp + i * (size_t) k, (size_t) nrhs * sizeof(double));
     free(tmp);
     CU(e);
-    return ACG_SUCCESS;
-}
-
-static int push_mstate(struct solvectx *c, const struct acgb200_mstate *ms)
-{
-    int *errcode = c->errcode;
-    CU(cudaStreamSynchronize(c->pv->stream));
-    *c->pv->h_ms = *ms;
-    CU(cudaMemcpyAsync(c->pv->d_ms, c->pv->h_ms, sizeof(*ms), cudaMemcpyHostToDevice, c->pv->stream));
-    CU(cudaStreamSynchronize(c->pv->stream));
-    return ACG_SUCCESS;
-}
-
-static int pull_mstate(struct solvectx *c, struct acgb200_mstate *ms)
-{
-    int *errcode = c->errcode;
-    CU(cudaMemcpyAsync(c->pv->h_ms, c->pv->d_ms, sizeof(*ms), cudaMemcpyDeviceToHost, c->pv->stream));
-    CU(cudaStreamSynchronize(c->pv->stream));
-    *ms = *c->pv->h_ms;
     return ACG_SUCCESS;
 }
 
@@ -1591,14 +1627,13 @@ int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acgsymcsrma
     cfg_load();
     struct priv *pv = priv_of(cg);
     if (!pv) return ACG_ERR_INVALID_VALUE;
-    if (!have_multi_kernels() || pv->nghost > 0 || pv->commsize > 1 || (A && A->nghostrows > 0))
-        return ACG_ERR_NOT_SUPPORTED;      /* one GPU, whole matrix */
+    if (!have_multi_kernels() || !one_gpu(pv, A)) return ACG_ERR_NOT_SUPPORTED;
     if (nrhs < 1 || nrhs > ACGB200_MAXK || !B || !X || maxits < 0) return ACG_ERR_INVALID_VALUE;
     const int K = block_width(nrhs), n = pv->nowned;
     OK(ensure_blocks(pv, cg, K, errcode));
     struct solvectx c;
     memset(&c, 0, sizeof(c));
-    c.cg = cg; c.pv = pv; c.errcode = errcode; c.mk = K;
+    c.cg = cg; c.pv = pv; c.errcode = errcode; c.mk = K; c.kind = KIND_MULTI;
     c.d_b = pv->d_mb; c.d_x = pv->d_mx;
     const double tb = wall();
     OK(upload_block_vec(pv, pv->d_mb, B, nrhs, K, errcode));
@@ -1612,40 +1647,27 @@ int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acgsymcsrma
     if (warmup > 0) {
         memset(&m, 0, sizeof(m));
         for (int j = 0; j < ACGB200_MAXK; j++) m.rr[0][j] = 1.0;
-        OK(push_mstate(&c, &m));
+        OK(scalars_push(&c, pv->d_ms, pv->h_ms, &m, sizeof(m)));
         memset(&h, 0, sizeof(h));
         h.maxits = warmup; h.ctrl[0].pad0 = (1 << K) - 1;
-        OK(push_state(&c, &h));
+        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
         c.d_x = pv->d_mr;
         for (int i = 0; i < warmup; i++) OK(multi_iteration(&c, i));
         c.d_x = pv->d_mx;
         KL(acgb200_dot_multi(n, K, pv->d_mb, &pv->d_ms->tmp[0], pv->stream));
         CU(cudaStreamSynchronize(pv->stream));
     }
-    if (cfg.profile) {
-        OK(evpool_reserve(&pv->gemv, 2 * (maxits + 2)));
-        OK(evpool_reserve(&pv->blas, 2 * (maxits + 2)));
-    }
-    pv->gemv.n = pv->blas.n = 0;
-
-    cg->nsolves++; cg->niterations = 0;
-    cg->bnrm2 = cg->r0nrm2 = cg->rnrm2 = cg->x0nrm2 = cg->dxnrm2 = INFINITY;
-    cg->maxits = maxits; cg->diffatol = 0; cg->diffrtol = 0;
-    cg->residualatol = residualatol; cg->residualrtol = residualrtol;
-    CU(cudaStreamSynchronize(pv->stream));
-    const double t0 = wall();
-    CU(cudaEventRecord(pv->ev_t0, pv->stream));
-    c.launches = 0;
+    OK(window_open(&c, maxits, residualatol, residualrtol, 0, 0));
 
     /* ||b_j|| ; r0 = B - A X0 with (r0_j,r0_j) folded in ; P = R */
     memset(&h, 0, sizeof(h));
-    OK(push_state(&c, &h));
+    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
     memset(&m, 0, sizeof(m));
-    OK(push_mstate(&c, &m));
+    OK(scalars_push(&c, pv->d_ms, pv->h_ms, &m, sizeof(m)));
     KL(acgb200_dot_multi(n, K, pv->d_mb, &pv->d_ms->tmp[0], pv->stream));
     OK(apply_A_multi(&c, pv->d_mx, pv->d_mr, pv->d_mb, SPMV_R_B_AX, &pv->d_ms->rr[0][0], 0));
     CU(cudaMemcpyAsync(pv->d_mp, pv->d_mr, (size_t) n * K * sizeof(double), cudaMemcpyDeviceToDevice, pv->stream));
-    OK(pull_mstate(&c, &m));
+    OK(scalars_pull(&c, pv->d_ms, pv->h_ms, &m, sizeof(m)));
     c.launches += 1;
     double bb[ACGB200_MAXK], rr0[ACGB200_MAXK], tol[ACGB200_MAXK], rtol_scaled[ACGB200_MAXK];
     unsigned mask = 0;
@@ -1663,36 +1685,26 @@ int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acgsymcsrma
     if (maxits > 0 && mask) {
         memset(&m, 0, sizeof(m));
         for (int j = 0; j < nrhs; j++) { m.tol[j] = tol[j]; m.rr[0][j] = rr0[j]; m.final_rr[j] = rr0[j]; }
-        OK(push_mstate(&c, &m));
+        OK(scalars_push(&c, pv->d_ms, pv->h_ms, &m, sizeof(m)));
         memset(&h, 0, sizeof(h));
         h.maxits = maxits; h.ctrl[0].pad0 = (int) mask;
-        OK(push_state(&c, &h));
-        OK(iterate(&c, maxits, poll, 2, multi_iteration));
-        OK(pull_state(&c, &h));
-        OK(pull_mstate(&c, &m));
+        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(iterate(&c, maxits, poll, multi_iteration));
+        OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_pull(&c, pv->d_ms, pv->h_ms, &m, sizeof(m)));
         cg->niterations = h.ctrl[0].iter;
         for (int j = 0; j < nrhs; j++)
             if (mask >> j & 1u) { nits[j] = m.nits[j]; conv[j] = m.conv[j]; rr[j] = m.final_rr[j]; }
     }
     cg->ntotaliterations += cg->niterations;
-    CU(cudaEventRecord(pv->ev_t1, pv->stream));
-    CU(cudaEventSynchronize(pv->ev_t1));
-    cg->tsolve += wall() - t0;
-    { float ms = 0; if (cudaEventElapsedTime(&ms, pv->ev_t0, pv->ev_t1) == cudaSuccess) pv->last_solve_ms = ms; }
+    OK(window_close(&c));
     account_multi(cg, pv, cg->niterations, K);
     cg->ngemv++; cg->ncopy += 1; cg->nnrm2 += 2 * nrhs;
-    pv->last_launches = c.launches;
-    if (cfg.profile) {
-        pv->last_spmv_ms = evpool_sum_ms(&pv->gemv); pv->last_spmv_n = pv->gemv.n / 2;
-        pv->last_blas_ms = evpool_sum_ms(&pv->blas);
-        cg->tgemv += 1e-3 * pv->last_spmv_ms;
-        cg->taxpy += 1e-3 * pv->last_blas_ms;
-    }
     double sb = 0, sr0 = 0, sr = 0;
     int status = ACG_SUCCESS;
     for (int j = 0; j < nrhs; j++) {
         sb += bb[j]; sr0 += rr0[j]; sr += rr[j];
-        if (!conv[j] && !(residualatol == 0 && rtol_scaled[j] == 0)) status = ACG_ERR_NOT_CONVERGED;   /* :1099-1107 per column */
+        if (not_converged(conv[j], residualatol, rtol_scaled[j])) status = ACG_ERR_NOT_CONVERGED;      /* per column */
         if (stats) {
             stats[j].niterations = nits[j]; stats[j].converged = conv[j];
             stats[j].bnrm2 = sqrt(bb[j]); stats[j].r0nrm2 = sqrt(rr0[j]); stats[j].rnrm2 = sqrt(rr[j]);
@@ -1714,25 +1726,6 @@ int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acgsymcsrma
 static int have_shift_kernels(void)
 {
     return have_multi_kernels() && acgb200_shift_setup && acgb200_cg_shift_update;
-}
-
-static int push_sstate(struct solvectx *c, const struct acgb200_sstate *ss)
-{
-    int *errcode = c->errcode;
-    CU(cudaStreamSynchronize(c->pv->stream));
-    *c->pv->h_ss = *ss;
-    CU(cudaMemcpyAsync(c->pv->d_ss, c->pv->h_ss, sizeof(*ss), cudaMemcpyHostToDevice, c->pv->stream));
-    CU(cudaStreamSynchronize(c->pv->stream));
-    return ACG_SUCCESS;
-}
-
-static int pull_sstate(struct solvectx *c, struct acgb200_sstate *ss)
-{
-    int *errcode = c->errcode;
-    CU(cudaMemcpyAsync(c->pv->h_ss, c->pv->d_ss, sizeof(*ss), cudaMemcpyDeviceToHost, c->pv->stream));
-    CU(cudaStreamSynchronize(c->pv->stream));
-    *ss = *c->pv->h_ss;
-    return ACG_SUCCESS;
 }
 
 /* the state of iteration 0: zeta_0 = zeta_{-1} = 1, alpha_{-1} = 1, beta_{-1} = 0 */
@@ -1784,8 +1777,7 @@ int acgsolvercuda_solve_shifted(struct acgsolvercuda *cg, const struct acgsymcsr
     cfg_load();
     struct priv *pv = priv_of(cg);
     if (!pv) return ACG_ERR_INVALID_VALUE;
-    if (!have_shift_kernels() || pv->nghost > 0 || pv->commsize > 1 || (A && A->nghostrows > 0))
-        return ACG_ERR_NOT_SUPPORTED;      /* one GPU, whole matrix */
+    if (!have_shift_kernels() || !one_gpu(pv, A)) return ACG_ERR_NOT_SUPPORTED;
     if (nshifts < 1 || nshifts > ACGB200_MAXK || !shifts || !b || !X || maxits < 0) return ACG_ERR_INVALID_VALUE;
     for (int j = 0; j < nshifts; j++) if (!(isfinite(shifts[j]) && shifts[j] >= 0)) return ACG_ERR_INVALID_VALUE;
     const int K = block_width(nshifts), n = pv->nowned;
@@ -1796,7 +1788,7 @@ int acgsolvercuda_solve_shifted(struct acgsolvercuda *cg, const struct acgsymcsr
     }
     struct solvectx c;
     memset(&c, 0, sizeof(c));
-    c.cg = cg; c.pv = pv; c.errcode = errcode; c.mk = K; c.shifted = 1;
+    c.cg = cg; c.pv = pv; c.errcode = errcode; c.mk = K; c.kind = KIND_SHIFTED;
     /* b lives in the first n entries of the B block, which this loop does not otherwise use */
     double *const d_b = pv->d_mb;
     c.d_b = d_b; c.d_x = pv->d_mx;
@@ -1813,33 +1805,20 @@ int acgsolvercuda_solve_shifted(struct acgsolvercuda *cg, const struct acgsymcsr
     if (warmup > 0) {
         KL(acgb200_shift_setup(n, K, d_b, cg->d_r, cg->d_p, pv->d_mr, pv->d_mp, pv->stream));
         sstate_init(&ss, nshifts, shifts, 0.0, 1.0);
-        OK(push_sstate(&c, &ss));
+        OK(scalars_push(&c, pv->d_ss, pv->h_ss, &ss, sizeof(ss)));
         memset(&h, 0, sizeof(h));
         h.maxits = warmup; h.rr_loc[0] = h.rr[0] = 1.0; h.ctrl[0].pad0 = (int) all;
-        OK(push_state(&c, &h));
+        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
         c.d_x = pv->d_mr;
         for (int i = 0; i < warmup; i++) OK(shifted_iteration(&c, i));
         c.d_x = pv->d_mx;
         CU(cudaStreamSynchronize(pv->stream));
     }
-    if (cfg.profile) {
-        OK(evpool_reserve(&pv->gemv, 2 * (maxits + 2)));
-        OK(evpool_reserve(&pv->blas, 2 * (maxits + 2)));
-    }
-    pv->gemv.n = pv->blas.n = 0;
-
-    cg->nsolves++; cg->niterations = 0;
-    cg->bnrm2 = cg->r0nrm2 = cg->rnrm2 = cg->x0nrm2 = cg->dxnrm2 = INFINITY;
-    cg->maxits = maxits; cg->diffatol = 0; cg->diffrtol = 0;
-    cg->residualatol = residualatol; cg->residualrtol = residualrtol;
-    CU(cudaStreamSynchronize(pv->stream));
-    const double t0 = wall();
-    CU(cudaEventRecord(pv->ev_t0, pv->stream));
-    c.launches = 0;
+    OK(window_open(&c, maxits, residualatol, residualrtol, 0, 0));
 
     /* r0 = p0 = b (x0 = 0 for every shift), X = 0, P_j = b ; ||b|| */
     memset(&h, 0, sizeof(h));
-    OK(push_state(&c, &h));
+    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
     KL(acgb200_shift_setup(n, K, d_b, cg->d_r, cg->d_p, pv->d_mx, pv->d_mp, pv->stream));
     KL(acgb200_dot(n, d_b, d_b, &pv->d_st->tmp_loc[0], pv->stream));
     double bb = 0;
@@ -1855,35 +1834,25 @@ int acgsolvercuda_solve_shifted(struct acgsolvercuda *cg, const struct acgsymcsr
     for (int j = 0; j < nshifts; j++) { nits[j] = 0; conv[j] = !(mask >> j & 1u); rn[j] = bnrm2; }
     if (maxits > 0 && mask) {
         sstate_init(&ss, nshifts, shifts, tol, bnrm2);
-        OK(push_sstate(&c, &ss));
+        OK(scalars_push(&c, pv->d_ss, pv->h_ss, &ss, sizeof(ss)));
         memset(&h, 0, sizeof(h));
         h.maxits = maxits; h.rr_loc[0] = h.rr[0] = bb; h.ctrl[0].pad0 = (int) mask;
-        OK(push_state(&c, &h));
-        OK(iterate(&c, maxits, tol > 0, 3, shifted_iteration));
-        OK(pull_state(&c, &h));
-        OK(pull_sstate(&c, &ss));
+        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(iterate(&c, maxits, tol > 0, shifted_iteration));
+        OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_pull(&c, pv->d_ss, pv->h_ss, &ss, sizeof(ss)));
         cg->niterations = h.ctrl[0].iter;
         for (int j = 0; j < nshifts; j++) { nits[j] = ss.nits[j]; conv[j] = ss.conv[j]; rn[j] = ss.final_rnrm2[j]; }
     }
     cg->ntotaliterations += cg->niterations;
-    CU(cudaEventRecord(pv->ev_t1, pv->stream));
-    CU(cudaEventSynchronize(pv->ev_t1));
-    cg->tsolve += wall() - t0;
-    { float ms = 0; if (cudaEventElapsedTime(&ms, pv->ev_t0, pv->ev_t1) == cudaSuccess) pv->last_solve_ms = ms; }
+    OK(window_close(&c));
     account_shifted(cg, pv, cg->niterations, nshifts);
     cg->ncopy += 2; cg->nnrm2++;
-    pv->last_launches = c.launches;
-    if (cfg.profile) {
-        pv->last_spmv_ms = evpool_sum_ms(&pv->gemv); pv->last_spmv_n = pv->gemv.n / 2;
-        pv->last_blas_ms = evpool_sum_ms(&pv->blas);
-        cg->tgemv += 1e-3 * pv->last_spmv_ms;
-        cg->taxpy += 1e-3 * pv->last_blas_ms;
-    }
     double sr = 0;
     int status = ACG_SUCCESS;
     for (int j = 0; j < nshifts; j++) {
         sr += rn[j] * rn[j];
-        if (!conv[j] && !(residualatol == 0 && rtol_scaled == 0)) status = ACG_ERR_NOT_CONVERGED;   /* :1099-1107 per shift */
+        if (not_converged(conv[j], residualatol, rtol_scaled)) status = ACG_ERR_NOT_CONVERGED;      /* per shift */
         if (stats) {
             stats[j].niterations = nits[j]; stats[j].converged = conv[j];
             stats[j].bnrm2 = bnrm2; stats[j].r0nrm2 = bnrm2; stats[j].rnrm2 = rn[j];
@@ -1907,32 +1876,13 @@ static int have_minres_kernels(void)
     return acgb200_minres_setup && acgb200_minres_lanczos && acgb200_minres_update;
 }
 
-static int push_nstate(struct solvectx *c, const struct acgb200_nstate *ns)
-{
-    int *errcode = c->errcode;
-    CU(cudaStreamSynchronize(c->pv->stream));
-    *c->pv->h_ns = *ns;
-    CU(cudaMemcpyAsync(c->pv->d_ns, c->pv->h_ns, sizeof(*ns), cudaMemcpyHostToDevice, c->pv->stream));
-    CU(cudaStreamSynchronize(c->pv->stream));
-    return ACG_SUCCESS;
-}
-
-static int pull_nstate(struct solvectx *c, struct acgb200_nstate *ns)
-{
-    int *errcode = c->errcode;
-    CU(cudaMemcpyAsync(c->pv->h_ns, c->pv->d_ns, sizeof(*ns), cudaMemcpyDeviceToHost, c->pv->stream));
-    CU(cudaStreamSynchronize(c->pv->stream));
-    *ns = *c->pv->h_ns;
-    return ACG_SUCCESS;
-}
-
 /* r0 = b - A x into d_r with (r0,r0) folded in; *r0nrm2 = ||r0|| */
 static int minres_residual(struct solvectx *c, double *r0nrm2)
 {
     struct priv *pv = c->pv;
     struct acgb200_devstate h;
     memset(&h, 0, sizeof(h));
-    OK(push_state(c, &h));
+    OK(scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h)));
     double rr = 0;
     OK(apply_A(c, c->d_x, c->d_x, c->cg->d_r, c->d_b, SPMV_R_B_AX, &pv->d_st->tmp_loc[0], 0, 0, 0, -1));
     OK(reduce_to_host(c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &rr));
@@ -1952,11 +1902,11 @@ static int minres_start(struct solvectx *c, int maxits, double tol, double beta1
     struct acgb200_nstate ns;
     memset(&ns, 0, sizeof(ns));
     ns.beta[0] = beta1; ns.cs[0] = -1.0; ns.phibar[0] = beta1;
-    OK(push_nstate(c, &ns));
+    OK(scalars_push(c, pv->d_ns, pv->h_ns, &ns, sizeof(ns)));
     struct acgb200_devstate h;
     memset(&h, 0, sizeof(h));
     h.maxits = maxits; h.tol = tol;
-    return push_state(c, &h);
+    return scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h));
 }
 
 /* iteration k: t = A v_k (+ alpha_k), u = t - alpha_k v_k - beta_k v_{k-1} (+ (u,u)), then the rotation, w_k, x
@@ -2000,15 +1950,12 @@ int acgsolvercuda_solve_minres(struct acgsolvercuda *cg, const struct acgsymcsrm
     cfg_load();
     struct priv *pv = priv_of(cg);
     if (!pv || !A || !b || !x) return ACG_ERR_INVALID_VALUE;
-    if (!have_minres_kernels() || pv->nghost > 0 || pv->commsize > 1 || A->nghostrows > 0)
-        return ACG_ERR_NOT_SUPPORTED;      /* one GPU, whole matrix */
+    if (!have_minres_kernels() || !one_gpu(pv, A)) return ACG_ERR_NOT_SUPPORTED;
     if (maxits < 0) return ACG_ERR_INVALID_VALUE;
-    struct acgcomm null;
-    memset(&null, 0, sizeof(null));
-    null.type = acgcomm_null;
+    struct acgcomm null = null_comm();
     struct solvectx c;
     OK(solve_begin(&c, cg, A, b, x, 0.0, 0.0, &null, 0, errcode));
-    c.minres = 1;
+    c.kind = KIND_MINRES;
     const int n = pv->nowned;
     if (!pv->d_ns) {
         CU(cudaMalloc((void **) &pv->d_ns, sizeof(*pv->d_ns)));
@@ -2025,30 +1972,13 @@ int acgsolvercuda_solve_minres(struct acgsolvercuda *cg, const struct acgsymcsrm
         OK(minres_residual(&c, &beta1));
         OK(minres_start(&c, warmup, 0.0, beta1));
         for (int i = 0; i < warmup; i++) OK(minres_iteration(&c, i));
-        const double tb = wall();
-        const size_t nx = (size_t) (x->num_nonzeros < pv->nvec ? x->num_nonzeros : pv->nvec);
-        CU(cudaMemcpyAsync(c.d_x, x->x, nx * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
-        CU(cudaStreamSynchronize(pv->stream));
-        pv->last_h2d_ms += 1e3 * (wall() - tb);
+        OK(upload_x0(&c, x));
     }
-    if (cfg.profile) {
-        OK(evpool_reserve(&pv->gemv, 2 * (maxits + 2)));
-        OK(evpool_reserve(&pv->blas, 2 * (maxits + 2)));
-    }
-    pv->gemv.n = pv->blas.n = 0;
-
-    cg->nsolves++; cg->niterations = 0;
-    cg->bnrm2 = cg->r0nrm2 = cg->rnrm2 = cg->x0nrm2 = cg->dxnrm2 = INFINITY;
-    cg->maxits = maxits; cg->diffatol = 0; cg->diffrtol = 0;
-    cg->residualatol = residualatol; cg->residualrtol = residualrtol;
-    CU(cudaStreamSynchronize(pv->stream));
-    const double t0 = wall();
-    CU(cudaEventRecord(pv->ev_t0, pv->stream));
-    c.launches = 0;
+    OK(window_open(&c, maxits, residualatol, residualrtol, 0, 0));
 
     /* ||b|| ; r0 = b - A x0 and beta_1 = ||r0|| */
     memset(&h, 0, sizeof(h));
-    OK(push_state(&c, &h));
+    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
     double bb = 0, beta1 = 0;
     KL(acgb200_dot(n, c.d_b, c.d_b, &pv->d_st->tmp_loc[0], pv->stream));
     OK(reduce_to_host(&c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &bb));
@@ -2064,30 +1994,17 @@ int acgsolvercuda_solve_minres(struct acgsolvercuda *cg, const struct acgsymcsrm
     /* beta_1 = 0: x0 solves the system, there is no Krylov space to build */
     if (!converged && maxits > 0 && beta1 > 0) {
         OK(minres_start(&c, maxits, tol, beta1));
-        OK(iterate(&c, maxits, tol > 0, 4, minres_iteration));
-        OK(pull_state(&c, &h));
-        OK(pull_nstate(&c, &ns));
+        OK(iterate(&c, maxits, tol > 0, minres_iteration));
+        OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_pull(&c, pv->d_ns, pv->h_ns, &ns, sizeof(ns)));
         cg->niterations = h.ctrl[0].iter;
         cg->rnrm2 = ns.phibar[cg->niterations & 1];
         converged = tol > 0 && cg->rnrm2 < tol;
         cg->ntotaliterations += cg->niterations;
     }
-    CU(cudaEventRecord(pv->ev_t1, pv->stream));
-    CU(cudaEventSynchronize(pv->ev_t1));
-    cg->tsolve += wall() - t0;
-    { float ms = 0; if (cudaEventElapsedTime(&ms, pv->ev_t0, pv->ev_t1) == cudaSuccess) pv->last_solve_ms = ms; }
+    OK(window_close(&c));
     account_minres(cg, pv, cg->niterations);
-    pv->last_launches = c.launches;
-    pv->last_fused = 0;
-    if (cfg.profile) {
-        pv->last_spmv_ms = evpool_sum_ms(&pv->gemv); pv->last_spmv_n = pv->gemv.n / 2;
-        pv->last_blas_ms = evpool_sum_ms(&pv->blas);
-        cg->tgemv += 1e-3 * pv->last_spmv_ms;
-        cg->taxpy += 1e-3 * pv->last_blas_ms;
-    }
-    int status = ACG_SUCCESS;
-    if (!converged && !(residualatol == 0 && rtol_scaled == 0)) status = ACG_ERR_NOT_CONVERGED;   /* :1099-1107 */
-    return solve_end(&c, x, status);
+    return solve_end(&c, x, not_converged(converged, residualatol, rtol_scaled) ? ACG_ERR_NOT_CONVERGED : ACG_SUCCESS);
 }
 
 /* ------------------------------------------------------------------------ */
@@ -2127,25 +2044,6 @@ static float *mixed_vec(const struct priv *pv, int i)     /* 0 r, 1 p, 2 t, 3 y 
     return pv->d_f32 + (size_t) i * (((size_t) pv->nowned + 2) & ~(size_t) 1);
 }
 
-static int push_xstate(struct solvectx *c, const struct acgb200_xstate *xs)
-{
-    int *errcode = c->errcode;
-    CU(cudaStreamSynchronize(c->pv->stream));
-    *c->pv->h_xs = *xs;
-    CU(cudaMemcpyAsync(c->pv->d_xs, c->pv->h_xs, sizeof(*xs), cudaMemcpyHostToDevice, c->pv->stream));
-    CU(cudaStreamSynchronize(c->pv->stream));
-    return ACG_SUCCESS;
-}
-
-static int pull_xstate(struct solvectx *c, struct acgb200_xstate *xs)
-{
-    int *errcode = c->errcode;
-    CU(cudaMemcpyAsync(c->pv->h_xs, c->pv->d_xs, sizeof(*xs), cudaMemcpyDeviceToHost, c->pv->stream));
-    CU(cudaStreamSynchronize(c->pv->stream));
-    *xs = *c->pv->h_xs;
-    return ACG_SUCCESS;
-}
-
 /* the fp32 product t = fl32(A p) with (p, t) into acc; gated: by ctrl[0] */
 static int apply_A_f32(struct solvectx *c, const float *x, float *y, double *acc, int gated)
 {
@@ -2172,7 +2070,7 @@ static int mixed_residual(struct solvectx *c, double *rr)
     struct priv *pv = c->pv;
     struct acgb200_devstate h;
     memset(&h, 0, sizeof(h));
-    OK(push_state(c, &h));
+    OK(scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h)));
     *rr = 0;
     OK(apply_A(c, c->d_x, c->d_x, c->cg->d_r, c->d_b, SPMV_R_B_AX, &pv->d_st->tmp_loc[0], 0, 0, 0, -1));
     return reduce_to_host(c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, rr);
@@ -2199,11 +2097,11 @@ static int mixed_start(struct solvectx *c, int maxits, double tol, double rr64)
     memset(&xs, 0, sizeof(xs));
     xs.rho[0] = ldexp(rr64, -2 * e); xs.mx[0] = sqrt(xs.rho[0]); xs.sigma[0] = ldexp(1.0, e);
     xs.last_rr64 = rr64;
-    OK(push_xstate(c, &xs));
+    OK(scalars_push(c, pv->d_xs, pv->h_xs, &xs, sizeof(xs)));
     struct acgb200_devstate h;
     memset(&h, 0, sizeof(h));
     h.maxits = maxits; h.tol = tol;
-    return push_state(c, &h);
+    return scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h));
 }
 
 /* iteration k: t = fl32(A p) (+ pi), r -= alpha t (+ rho'), y and p (or the fold), the fp64 residual and
@@ -2247,15 +2145,12 @@ int acgsolvercuda_solve_mixed(struct acgsolvercuda *cg, const struct acgsymcsrma
     cfg_load();
     struct priv *pv = priv_of(cg);
     if (!pv || !A || !b || !x) return ACG_ERR_INVALID_VALUE;
-    if (!have_mixed_kernels() || pv->nghost > 0 || pv->commsize > 1 || A->nghostrows > 0)
-        return ACG_ERR_NOT_SUPPORTED;      /* one GPU, whole matrix */
+    if (!have_mixed_kernels() || !one_gpu(pv, A)) return ACG_ERR_NOT_SUPPORTED;
     if (maxits < 0) return ACG_ERR_INVALID_VALUE;
-    struct acgcomm null;
-    memset(&null, 0, sizeof(null));
-    null.type = acgcomm_null;
+    struct acgcomm null = null_comm();
     struct solvectx c;
     OK(solve_begin(&c, cg, A, b, x, 0.0, 0.0, &null, 0, errcode));
-    c.mixed = 1;
+    c.kind = KIND_MIXED;
     const int n = pv->nowned;
     OK(mixed_alloc(pv, cg, errcode));
     struct acgb200_devstate h;
@@ -2269,31 +2164,13 @@ int acgsolvercuda_solve_mixed(struct acgsolvercuda *cg, const struct acgsymcsrma
             OK(mixed_start(&c, warmup, 0.0, rr));
             for (int i = 0; i < warmup; i++) OK(mixed_iteration(&c, i));
         }
-        const double tb = wall();
-        const size_t nx = (size_t) (x->num_nonzeros < pv->nvec ? x->num_nonzeros : pv->nvec);
-        CU(cudaMemcpyAsync(c.d_x, x->x, nx * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
-        CU(cudaStreamSynchronize(pv->stream));
-        pv->last_h2d_ms += 1e3 * (wall() - tb);
+        OK(upload_x0(&c, x));
     }
-    if (cfg.profile) {
-        OK(evpool_reserve(&pv->gemv, 2 * (maxits + 2)));
-        OK(evpool_reserve(&pv->blas, 2 * (maxits + 2)));
-    }
-    pv->gemv.n = pv->blas.n = 0;
-
-    cg->nsolves++; cg->niterations = 0;
-    cg->bnrm2 = cg->r0nrm2 = cg->rnrm2 = cg->x0nrm2 = cg->dxnrm2 = INFINITY;
-    cg->maxits = maxits; cg->diffatol = 0; cg->diffrtol = 0;
-    cg->residualatol = residualatol; cg->residualrtol = residualrtol;
-    pv->last_mixed_updates = 0;
-    CU(cudaStreamSynchronize(pv->stream));
-    const double t0 = wall();
-    CU(cudaEventRecord(pv->ev_t0, pv->stream));
-    c.launches = 0;
+    OK(window_open(&c, maxits, residualatol, residualrtol, 0, 0));
 
     /* ||b|| ; r0 = b - A x0 in fp64 */
     memset(&h, 0, sizeof(h));
-    OK(push_state(&c, &h));
+    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
     double bb = 0, rr0 = 0;
     KL(acgb200_dot(n, c.d_b, c.d_b, &pv->d_st->tmp_loc[0], pv->stream));
     OK(reduce_to_host(&c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &bb));
@@ -2310,9 +2187,9 @@ int acgsolvercuda_solve_mixed(struct acgsolvercuda *cg, const struct acgsymcsrma
     /* ||r0|| = 0: x0 solves the system */
     if (!converged && maxits > 0 && rr0 > 0) {
         OK(mixed_start(&c, maxits, tol, rr0));
-        OK(iterate(&c, maxits, 1, 5, mixed_iteration));
-        OK(pull_state(&c, &h));
-        OK(pull_xstate(&c, &xs));
+        OK(iterate(&c, maxits, 1, mixed_iteration));
+        OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_pull(&c, pv->d_xs, pv->h_xs, &xs, sizeof(xs)));
         cg->niterations = h.ctrl[0].iter;
         nupdates = xs.nupdates;
         if (xs.conv || xs.breakdown) {
@@ -2330,23 +2207,10 @@ int acgsolvercuda_solve_mixed(struct acgsolvercuda *cg, const struct acgsymcsrma
         converged = tol > 0 && cg->rnrm2 < tol;
         cg->ntotaliterations += cg->niterations;
     }
-    CU(cudaEventRecord(pv->ev_t1, pv->stream));
-    CU(cudaEventSynchronize(pv->ev_t1));
-    cg->tsolve += wall() - t0;
-    { float ms = 0; if (cudaEventElapsedTime(&ms, pv->ev_t0, pv->ev_t1) == cudaSuccess) pv->last_solve_ms = ms; }
+    OK(window_close(&c));
     account_mixed(cg, pv, cg->niterations, nupdates);
-    pv->last_launches = c.launches;
-    pv->last_fused = 0;
     pv->last_mixed_updates = nupdates;
-    if (cfg.profile) {
-        pv->last_spmv_ms = evpool_sum_ms(&pv->gemv); pv->last_spmv_n = pv->gemv.n / 2;
-        pv->last_blas_ms = evpool_sum_ms(&pv->blas);
-        cg->tgemv += 1e-3 * pv->last_spmv_ms;
-        cg->taxpy += 1e-3 * pv->last_blas_ms;
-    }
-    int status = ACG_SUCCESS;
-    if (!converged && !(residualatol == 0 && rtol_scaled == 0)) status = ACG_ERR_NOT_CONVERGED;   /* :1099-1107 */
-    return solve_end(&c, x, status);
+    return solve_end(&c, x, not_converged(converged, residualatol, rtol_scaled) ? ACG_ERR_NOT_CONVERGED : ACG_SUCCESS);
 }
 
 /* ------------------------------------------------------------------------ */
@@ -2443,12 +2307,12 @@ int acgsolvercuda_solve_pipelined(
     OK(ensure_vec(&cg->q, &cg->d_q, A, pv->nvec, errcode));
     OK(ensure_vec(&cg->z, &cg->d_z, A, pv->nvec, errcode));
 
+    c.kind = KIND_PIPELINED;
     c.p2p = c.multi && pv->p2p.enabled && cfg.p2p;
     /* one kernel per iteration: one GPU, mirrored diagonals for the slice rows, all other rows in tiles */
     const struct acgb200_spmvplan *pl = &pv->plan;
     c.fused = cfg.pcg_fused && !c.multi && pv->nghost == 0 && pv->nborder == 0 && pl->symdiag_nd > 0 && pl->pcg_grid > 0
               && pl->nmtiles == 0 && pl->nmed == 0 && pl->nlong == 0;
-    pv->last_fused = c.fused;
     if (c.fused && !pv->d_w2) {
         CU(cudaMalloc((void **) &pv->d_w2, ((size_t) pv->nvec + 2) * sizeof(double)));
         CU(cudaMemsetAsync(pv->d_w2, 0, ((size_t) pv->nvec + 2) * sizeof(double), pv->stream));
@@ -2458,7 +2322,7 @@ int acgsolvercuda_solve_pipelined(
         memset(&h, 0, sizeof(h));
         h.maxits = warmup;
         for (int s = 0; s < 2; s++) { h.gd_loc[s][0] = h.gd[s][0] = 1; h.gd_loc[s][1] = h.gd[s][1] = 1; h.prev[s][0] = h.prev[s][1] = INFINITY; }
-        OK(push_state(&c, &h));
+        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
         double *xsave = c.d_x; c.d_x = cg->d_r;
         if (c.p2p) {
             OK(acgb200_p2p_begin(&pv->p2p, warmup, pv->stream));
@@ -2470,29 +2334,15 @@ int acgsolvercuda_solve_pipelined(
         KL(acgb200_dot2(n, cg->d_r, cg->d_w, &st->tmp_loc[0], pv->stream));
         CU(cudaStreamSynchronize(pv->stream));
     }
-    if (cfg.profile) {
-        OK(evpool_reserve(&pv->gemv, 2 * (maxits + 3)));
-        OK(evpool_reserve(&pv->blas, 2 * (maxits + 3)));
-    }
-    pv->gemv.n = pv->blas.n = 0;
     /* z = t = p = 0 (acg/cgcuda.c:1516-1522) */
     CU(cudaMemsetAsync(cg->d_z, 0, obytes, pv->stream));
     CU(cudaMemsetAsync(cg->d_t, 0, obytes, pv->stream));
     CU(cudaMemsetAsync(cg->d_p, 0, obytes, pv->stream));
     CU(cudaMemsetAsync(cg->d_w, 0, ((size_t) pv->nvec + 2) * sizeof(double), pv->stream));
-
-    cg->nsolves++; cg->niterations = 0;
-    cg->bnrm2 = cg->r0nrm2 = cg->rnrm2 = cg->x0nrm2 = cg->dxnrm2 = INFINITY;
-    cg->maxits = maxits; cg->diffatol = diffatol; cg->diffrtol = diffrtol;
-    cg->residualatol = residualatol; cg->residualrtol = residualrtol;
-    OK(acgcomm_barrier(pv->stream, comm, errcode));
-    CU(cudaStreamSynchronize(pv->stream));
-    const double t0 = wall();
-    CU(cudaEventRecord(pv->ev_t0, pv->stream));
-    c.launches = 0;
+    OK(window_open(&c, maxits, residualatol, residualrtol, diffatol, diffrtol));
 
     memset(&h, 0, sizeof(h));
-    OK(push_state(&c, &h));
+    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
     double bb = 0, gd0[2] = { 0, 0 };
     KL(acgb200_dot(n, c.d_b, c.d_b, &st->tmp_loc[0], pv->stream));
     OK(reduce_to_host(&c, &st->tmp_loc[0], &st->tmp[0], 1, &bb));
@@ -2517,14 +2367,14 @@ int acgsolvercuda_solve_pipelined(
         h.gd_loc[0][0] = h.gd[0][0] = gd0[0];
         h.gd_loc[0][1] = h.gd[0][1] = gd0[1];
         h.prev[0][0] = h.prev[0][1] = INFINITY;                    /* acg/cgcuda.c:1513-1514 */
-        OK(push_state(&c, &h));
+        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
         if (c.p2p) {
             /* w_0 goes to the neighbours' windows as exchange number 0 */
             OK(acgb200_p2p_begin(&pv->p2p, maxits, pv->stream));
             OK(post(&c, 0, 0, cg->d_w, -1, NULL, 0, 0, 0, 0));
         }
-        OK(iterate(&c, maxits, tol > 0, 1, pipelined_iteration));
-        OK(pull_state(&c, &h));
+        OK(iterate(&c, maxits, tol > 0, pipelined_iteration));
+        OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
         const struct acgb200_ctrl cw = h.ctrl[c.fused ? c.issued & 1 : 0];
         cg->niterations = cw.iter;
         converged = cw.done;
@@ -2536,11 +2386,7 @@ int acgsolvercuda_solve_pipelined(
         cg->rnrm2 = sqrt(g);
         cg->ntotaliterations += cg->niterations;
     }
-    CU(cudaEventRecord(pv->ev_t1, pv->stream));
-    CU(cudaEventSynchronize(pv->ev_t1));
-    const double t1 = wall();
-    cg->tsolve += t1 - t0;
-    { float ms = 0; if (cudaEventElapsedTime(&ms, pv->ev_t0, pv->ev_t1) == cudaSuccess) pv->last_solve_ms = ms; }
+    OK(window_close(&c));
     {
         const int64_t nits = cg->niterations, nnz = pv->fnnz + pv->onnz;
         const int64_t bgemv = nnz * 12 + (int64_t) n * 16 + (int64_t) (pv->nborder + pv->nghost) * 8 + (int64_t) pv->nvec * 8;
@@ -2553,16 +2399,7 @@ int acgsolvercuda_solve_pipelined(
             cg->nhalomsgs += (nits + 2) * cg->halo->nrecipients;
         }
     }
-    pv->last_launches = c.launches;
-    if (cfg.profile) {
-        pv->last_spmv_ms = evpool_sum_ms(&pv->gemv); pv->last_spmv_n = pv->gemv.n / 2;
-        pv->last_blas_ms = evpool_sum_ms(&pv->blas);
-        cg->tgemv += 1e-3 * pv->last_spmv_ms;
-        cg->taxpy += 1e-3 * pv->last_blas_ms;
-    }
-    int status = ACG_SUCCESS;
-    if (!converged && !(residualatol == 0 && rtol_scaled == 0)) status = ACG_ERR_NOT_CONVERGED;
-    return solve_end(&c, x, status);
+    return solve_end(&c, x, not_converged(converged, residualatol, rtol_scaled) ? ACG_ERR_NOT_CONVERGED : ACG_SUCCESS);
 }
 
 /* ------------------------------------------------------------------------ */
@@ -2878,7 +2715,7 @@ int acgsolvercuda_spmv_f32(struct acgsolvercuda *cg, const float *x, float *y, d
     int errcode_ = 0, *errcode = &errcode_;
     struct priv *pv = priv_of(cg);
     if (!pv || !x || !y) return ACG_ERR_INVALID_VALUE;
-    if (!have_mixed_kernels() || pv->nghost > 0 || pv->commsize > 1) return ACG_ERR_NOT_SUPPORTED;
+    if (!have_mixed_kernels() || !one_gpu(pv, NULL)) return ACG_ERR_NOT_SUPPORTED;
     OK(mixed_alloc(pv, cg, errcode));
     const int n = pv->nowned;
     struct acgb200_devstate *st = pv->d_st;
@@ -2907,7 +2744,7 @@ int acgsolvercuda_spmm_mode(struct acgsolvercuda *cg, int mode, int nrhs, const 
     int errcode_ = 0, *errcode = &errcode_;
     struct priv *pv = priv_of(cg);
     if (!pv) return ACG_ERR_INVALID_VALUE;
-    if (!have_multi_kernels() || pv->nghost > 0 || pv->commsize > 1) return ACG_ERR_NOT_SUPPORTED;
+    if (!have_multi_kernels() || !one_gpu(pv, NULL)) return ACG_ERR_NOT_SUPPORTED;
     if (nrhs < 1 || nrhs > ACGB200_MAXK || !X || !Y) return ACG_ERR_INVALID_VALUE;
     if (mode != SPMV_Y_AX && mode != SPMV_Y_AX_DOT && mode != SPMV_R_B_AX) return ACG_ERR_INVALID_VALUE;
     if (mode == SPMV_R_B_AX && !B) return ACG_ERR_INVALID_VALUE;

@@ -71,20 +71,31 @@ def solve_run(cg, A, arrays, M, n, run, seed):
 
 
 def alternate(A, n):
-    """solvempi, solve_minres and solve_mixed in turn on one solver; then solvempi on it against one on a
-    fresh solver, bitwise."""
+    """solvempi, solve_multi (two columns), solve_shifted (shifts 0 and 0.5), solve_minres and solve_mixed in
+    turn on one solver, with the reliable updates info() reports after each; then solvempi on it against one
+    on a fresh solver, bitwise."""
     cg = ab.SolverCuda(A)
     rng = np.random.default_rng(5)
     b = rng.standard_normal(n)
     bv = A.vector(); bv.x[:] = b
+    B = np.ascontiguousarray(np.stack([b, rng.standard_normal(n)], axis=1))
     out = {"steps": []}
-    for kind in ("mixed", "single", "minres", "mixed", "minres", "single", "mixed", "mixed"):
-        x = A.vector()
-        fn = {"mixed": cg.solve_mixed, "minres": cg.solve_minres, "single": cg.solvempi}[kind]
-        code = fn(bv, x, maxits=80, residualrtol=1e-8)
-        its = [int(cg.c.niterations)]
-        xs = x.x[:n].copy()
-        out["steps"].append({"kind": kind, "code": int(code), "its": its, "x": xs.tolist()})
+    for kind in ("mixed", "single", "multi", "minres", "mixed", "shifted", "minres", "single", "mixed", "multi",
+                 "shifted", "mixed"):
+        if kind == "multi":
+            X = np.zeros((n, 2))
+            code, st = cg.solve_multi(B, X, maxits=80, residualrtol=1e-8)
+            its, xs = [s["niterations"] for s in st], X.ravel()
+        elif kind == "shifted":
+            code, X, st = cg.solve_shifted(b, [0.0, 0.5], maxits=80, residualrtol=1e-8)
+            its, xs = [s["niterations"] for s in st], X.ravel()
+        else:
+            x = A.vector()
+            fn = {"mixed": cg.solve_mixed, "minres": cg.solve_minres, "single": cg.solvempi}[kind]
+            code = fn(bv, x, maxits=80, residualrtol=1e-8)
+            its, xs = [int(cg.c.niterations)], x.x[:n].copy()
+        out["steps"].append({"kind": kind, "code": int(code), "its": its, "x": xs.tolist(),
+                             "updates": int(cg.info()["mixed_reliable_updates"])})
     x1 = A.vector()
     cg.solvempi(bv, x1, maxits=80, residualrtol=1e-8)
     its1, r1 = int(cg.c.niterations), float(cg.c.rnrm2)

@@ -187,16 +187,25 @@ def test_path_selection(ab, options):
     assert inf["pcg_fused_min_bytes"] == inf["spmv_slice_rows"] * (8 * inf["spmv_symdiag_diagonals"] + 96)
     assert _path(ab, A, spmv_symdiag=0)["pcg_fused"] == 0
     assert _path(ab, A, pcg_fused=0)["pcg_fused"] == 0
-    # a classic solve after a fused one: spmv_min_bytes is the product's again
+    # a solve of any other kind after a fused one: spmv_min_bytes is the product's again
     options()
     cg = ab.SolverCuda(A)
     b = _rhs(A)
-    x = A.vector()
-    cg.solve_pipelined(b, x, maxits=8)
-    fused_bytes = cg.info()["spmv_min_bytes"]
-    cg.solvempi(b, x, maxits=8)
-    inf = cg.info()
-    assert inf["pcg_fused"] == 0 and inf["spmv_min_bytes"] < fused_bytes
+    n = A.c.nownedrows
+    B = np.ascontiguousarray(np.stack([b.x[:n], b.x[:n][::-1]], axis=1))
+    others = {"solvempi": lambda: cg.solvempi(b, A.vector(), maxits=8),
+              "solve_multi": lambda: cg.solve_multi(B, np.zeros((n, 2)), maxits=8),
+              "solve_shifted": lambda: cg.solve_shifted(b.x[:n], [0.0, 0.5], maxits=8),
+              "solve_minres": lambda: cg.solve_minres(b, A.vector(), maxits=8),
+              "solve_mixed": lambda: cg.solve_mixed(b, A.vector(), maxits=8)}
+    for name, solve in others.items():
+        cg.solve_pipelined(b, A.vector(), maxits=8)
+        inf = cg.info()
+        assert inf["pcg_fused"] == 1, name
+        fused_bytes = inf["spmv_min_bytes"]
+        solve()
+        inf = cg.info()
+        assert inf["pcg_fused"] == 0 and inf["spmv_min_bytes"] < fused_bytes, name
     cg.free()
     A.free()
     # full storage that is not exactly symmetric: no mirrored diagonals

@@ -3,9 +3,9 @@ stand-in of tests/hostsim, against the restatement of tests/mixedref.py: equal i
 reliable-update counts and codes, x within 1e-12 relative, and rnrm2 the fp64 residual of the x returned
 (against the exact residual of tests/exactref.py).
 Covers nonzero x0, rtol and atol stopping, maxits reached, maxits = 0 returning x0 bitwise, b = 0, warm-up
-0 and 2, (p, A p) = 0, rejected calls, and solvempi, solve_minres and solve_mixed alternating on one
-solver.  The stand-in keeps the kernels' roundings, scalar rules and slot discipline; the kernels
-themselves are checked on the H100 by test_gpu_mixed.py."""
+0 and 2, (p, A p) = 0, rejected calls, and solvempi, solve_multi, solve_shifted, solve_minres and
+solve_mixed alternating on one solver.  The stand-in keeps the kernels' roundings, scalar rules and slot
+discipline; the kernels themselves are checked on the H100 by test_gpu_mixed.py."""
 import json
 import os
 import subprocess
@@ -96,14 +96,19 @@ def test_zero_curvature(simlib):
 
 
 def test_alternating_with_other_solves(simlib):
-    """solve_mixed, solvempi and solve_minres in turn on one solver: every call gives what it gives alone
-    (the captured loops are replayed only for their own kind); a solvempi afterwards matches one on a fresh
-    solver bitwise."""
+    """solve_mixed, solvempi, solve_multi, solve_shifted and solve_minres in turn on one solver: every call
+    gives what it gives alone (the captured loops are replayed only for their own kind) and info() counts
+    the reliable updates of the last solve only; a solvempi afterwards matches one on a fresh solver
+    bitwise."""
     out = _run({"matrix": "27pt", "alternate": 1})
     alt = out["alternate"]
     first = {}
     for s in alt["steps"]:
         assert s["code"] == 0, s["kind"]
+        if s["kind"] == "mixed":
+            assert s["updates"] >= 1, s["kind"]
+        else:
+            assert s["updates"] == 0, s["kind"]
         first.setdefault(s["kind"], s)
         assert first[s["kind"]]["its"] == s["its"], s["kind"]
         assert first[s["kind"]]["x"] == s["x"], s["kind"]
