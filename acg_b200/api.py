@@ -131,7 +131,9 @@ class acgb200_info(C.Structure):
         [("spmv_symdiag_diagonals", C.c_int), ("spmv_symdiag_bytes", C.c_int64)] + \
         [("pcg_fused", C.c_int), ("pcg_fused_min_bytes", C.c_int64)] + \
         [("spmv_symdiag_codes", C.c_int), ("spmv_symdiag_code_bytes", C.c_int64)] + \
-        [("mixed_reliable_updates", C.c_int)]
+        [("mixed_reliable_updates", C.c_int)] + \
+        [("cheb_degree", C.c_int), ("cheb_est_iterations", C.c_int), ("cheb_breakdown", C.c_int),
+         ("cheb_lmin", C.c_double), ("cheb_lmax", C.c_double)]
 
 
 class acgb200_colstats(C.Structure):
@@ -163,7 +165,7 @@ EXPORTS = [
     "acgsolvercuda_init_constants", "acgsolvercuda_alpha", "acgsolvercuda_beta", "acgsolvercuda_daxpy_alpha",
     "acgsolvercuda_daxpy_minus_alpha", "acgsolvercuda_daypx_beta", "acgsolvercuda_pipelined_daxpy_fused",
     "acgsolvercuda_fwrite",
-    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_solve_multi", "acgsolvercuda_spmm_mode", "acgsolvercuda_solve_shifted", "acgsolvercuda_solve_minres", "acgsolvercuda_solve_mixed", "acgsolvercuda_spmv_f32", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
+    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_solve_multi", "acgsolvercuda_spmm_mode", "acgsolvercuda_solve_shifted", "acgsolvercuda_solve_minres", "acgsolvercuda_solve_mixed", "acgsolvercuda_spmv_f32", "acgsolvercuda_solve_chebyshev", "acgb200_cheb_interval_host", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
     "acgb200_nccl_unique_id", "acgb200_comm_init_rank", "acgb200_comm_destroy",
     "acgb200_host_register", "acgb200_host_unregister", "acgb200_spmv_plan_host", "acgb200_spmv_plan_host2", "acgb200_slices_host", "acgb200_symdiag_host", "acgb200_merge_plan_host", "acgb200_p2p_inverse_map", "acgb200_patterns_host", "acgb200_stencil_part",
     "acgb200_mtx_info", "acgb200_mtx_read", "acgb200_mtx_read_part", "acgb200_comm_matrix_row", "acgb200_partition_rows_grid", "acgb200_grid_factors", "acgb200_rmat_spd",
@@ -249,6 +251,10 @@ def lib() -> C.CDLL:
                                               C.c_double, C.c_double, C.c_int, P(acgb200_colstats)]
     L.acgsolvercuda_solve_minres.argtypes = [P(acgsolvercuda), P(acgsymcsrmatrix), P(acgvector), P(acgvector), C.c_int,
                                              C.c_double, C.c_double, C.c_int, P(C.c_int)]
+    L.acgsolvercuda_solve_chebyshev.argtypes = [P(acgsolvercuda), P(acgsymcsrmatrix), P(acgvector), P(acgvector), C.c_int,
+                                                C.c_double, C.c_double, C.c_int, C.c_double, C.c_double, C.c_int,
+                                                P(C.c_int)]
+    L.acgb200_cheb_interval_host.argtypes = [C.c_int, f64p, f64p, P(C.c_double), P(C.c_double)]
     L.acgsolvercuda_solve_mixed.argtypes = [P(acgsolvercuda), P(acgsymcsrmatrix), P(acgvector), P(acgvector), C.c_int,
                                             C.c_double, C.c_double, C.c_int, P(C.c_int)]
     f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
@@ -363,6 +369,17 @@ def symdiag_host(rowptr, colidx, cover_hi=None) -> dict:
     t = tab[:2 * no].reshape(no, 2)
     return dict(reason=SYMDIAG_REASONS[int(info[0])], O=o[:no].copy(), D=d[:nd].copy(), margin=int(info[3]),
                 stride=int(info[4]), voff=t[:, 0].copy(), coff=t[:, 1].copy())
+
+
+def cheb_interval_host(alpha, beta) -> tuple:
+    """acgb200_cheb_interval_host: the extreme eigenvalues (theta_min, theta_max) of the Lanczos tridiagonal
+    that acgsolvercuda_solve_chebyshev builds from k CG steps' alpha (k) and beta (k - 1)."""
+    alpha = np.ascontiguousarray(alpha, np.float64)
+    beta = np.ascontiguousarray(beta if len(beta) else [0.0], np.float64)
+    tmin, tmax = C.c_double(0), C.c_double(0)
+    _check(lib().acgb200_cheb_interval_host(len(alpha), alpha, beta, C.byref(tmin), C.byref(tmax)),
+           "acgb200_cheb_interval_host")
+    return tmin.value, tmax.value
 
 
 def spmv_plan_host(rowptr, colidx=None) -> dict:
@@ -806,6 +823,23 @@ class SolverCuda:
                                                 C.byref(err))
         if code != ACG_SUCCESS and (raise_on_not_converged or code != ACG_ERR_NOT_CONVERGED):
             raise AcgError(code, "acgsolvercuda_solve_minres", err.value)
+        return code
+
+    def solve_chebyshev(self, b, x, degree=2, lmin=0.0, lmax=0.0, maxits=100, residualatol=0.0, residualrtol=0.0,
+                        warmup=0, raise_on_not_converged=False):
+        """acgsolvercuda_solve_chebyshev: CG preconditioned with a degree-``degree`` Chebyshev polynomial in
+        D^-1 A over [lmin, lmax] (degree 0: Jacobi) on the solver's (positive definite) operator (one GPU, whole
+        matrix).  lmax = 0 estimates the upper bound from 10 Jacobi-PCG steps, lmin = 0 takes lmax / 10.  b, x:
+        Vectors as for ``solvempi``, x the initial guess, updated in place.  ``info()`` reports cheb_degree,
+        cheb_est_iterations, cheb_breakdown and the interval used (cheb_lmin, cheb_lmax).  Returns the code
+        like ``solve()``."""
+        err = C.c_int(0)
+        code = lib().acgsolvercuda_solve_chebyshev(C.byref(self.c), C.byref(self.A.c), C.byref(b.c), C.byref(x.c),
+                                                   int(degree), float(lmin), float(lmax), int(maxits),
+                                                   float(residualatol), float(residualrtol), int(warmup),
+                                                   C.byref(err))
+        if code != ACG_SUCCESS and (raise_on_not_converged or code != ACG_ERR_NOT_CONVERGED):
+            raise AcgError(code, "acgsolvercuda_solve_chebyshev", err.value)
         return code
 
     def solve_mixed(self, b, x, maxits=100, residualatol=0.0, residualrtol=0.0, warmup=0,

@@ -155,7 +155,7 @@ int acgb200_set_option(const char *key, int value)
 struct evpool { cudaEvent_t *ev; int n, cap; };
 
 /* the loops a solver runs; each has its own cached graph */
-enum solve_kind { KIND_CLASSIC, KIND_PIPELINED, KIND_MULTI, KIND_SHIFTED, KIND_MINRES, KIND_MIXED, NKINDS };
+enum solve_kind { KIND_CLASSIC, KIND_PIPELINED, KIND_MULTI, KIND_SHIFTED, KIND_MINRES, KIND_MIXED, KIND_CHEB, NKINDS };
 
 struct priv {
     const struct acgsolvercuda *key;
@@ -208,6 +208,15 @@ struct priv {
     int *d_franges;
     int nfranges, have_franges;
     int last_mixed_updates;
+    /* Chebyshev-preconditioned CG (acgsolvercuda_solve_chebyshev), made at the first such solve: its scalars
+     * and five vectors D^-1, z, res, d_0, d_1 (one allocation); baddiag: the diagonal entries that are <= 0 or
+     * non-finite (-1: not counted yet); cheb_graph_ab: the interval whose coefficients the cached graph holds */
+    struct acgb200_cstate *d_cs, *h_cs;
+    double *d_cvec;
+    int cheb_baddiag;
+    double cheb_graph_ab[2];
+    int last_cheb_degree, last_cheb_est, last_cheb_breakdown;
+    double last_cheb_lmin, last_cheb_lmax;
 };
 
 /* The public struct has no room for private state (its layout is the
@@ -312,6 +321,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
         cudaFree(pv->d_ss); cudaFreeHost(pv->h_ss);
         cudaFree(pv->d_ns); cudaFreeHost(pv->h_ns); cudaFree(pv->d_nw[0]); cudaFree(pv->d_nw[1]);
         cudaFree(pv->d_xs); cudaFreeHost(pv->h_xs); cudaFree(pv->d_f32); cudaFree(pv->d_franges);
+        cudaFree(pv->d_cs); cudaFreeHost(pv->h_cs); cudaFree(pv->d_cvec);
         cudaFree(pv->d_mx); cudaFree(pv->d_mb); cudaFree(pv->d_mr); cudaFree(pv->d_mp); cudaFree(pv->d_mt);
         if (pv->ev_ready) cudaEventDestroy(pv->ev_ready);
         if (pv->ev_halo) cudaEventDestroy(pv->ev_halo);
@@ -903,6 +913,11 @@ struct solvectx {
                                * alternates between ctrl[0] and ctrl[1] by iteration parity */
     int issued;               /* iterations iterate() issued, inactive ones included */
     double t0;                /* host clock at the start of the solve window */
+    /* Chebyshev loop: the degree, the fused inner step (acgb200_cheb_fused_step), the start's and the steps'
+     * coefficients, and the r and x the r/x kernel updates (x NULL: the estimate) */
+    int cheb_degree, cheb_fused;
+    double cheb_c0, cheb_c[ACGB200_CHEB_MAXDEG][2];
+    double *cheb_r, *cheb_x;
 };
 
 static int evpool_reserve(struct evpool *p, int n)
@@ -951,6 +966,8 @@ static int window_open(struct solvectx *c, int maxits, double atol, double rtol,
     /* what acgsolvercuda_info reports of the last solve, whichever entry point runs it */
     pv->last_fused = c->fused;
     pv->last_mixed_updates = 0;
+    pv->last_cheb_degree = pv->last_cheb_est = pv->last_cheb_breakdown = 0;
+    pv->last_cheb_lmin = pv->last_cheb_lmax = 0;
     pv->last_spmv_ms = pv->last_blas_ms = 0; pv->last_spmv_n = 0;
     OK(acgcomm_barrier(pv->stream, c->comm, errcode));
     CU(cudaStreamSynchronize(pv->stream));
@@ -1225,7 +1242,8 @@ static double threshold(double atol, double rtol, double r0nrm2)
 static int graph_signature(const struct solvectx *c)
 {
     return 1 | (c->multi ? 2 : 0) | (c->p2p ? 4 : 0) | (c->pv->p2p.h_desc.fuse ? 8 : 0) | (cfg.pdl ? 16 : 0)
-           | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0) | (c->mk << 8) | (c->fused ? 1 << 16 : 0);
+           | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0) | (c->mk << 8) | (c->fused ? 1 << 16 : 0)
+           | (c->cheb_degree << 18) | (c->cheb_fused ? 1 << 23 : 0);
 }
 
 static int capture_pair(struct solvectx *c, int (*issue)(struct solvectx *, int))
@@ -2214,6 +2232,365 @@ int acgsolvercuda_solve_mixed(struct acgsolvercuda *cg, const struct acgsymcsrma
 }
 
 /* ------------------------------------------------------------------------ */
+/* Chebyshev-preconditioned CG                                               */
+/* ------------------------------------------------------------------------ */
+
+/* the Chebyshev kernels are linked in (see ACGB200_MULTI_LAUNCHER, internal.h) */
+static int have_cheb_kernels(void)
+{
+    return acgb200_cheb_dinv && acgb200_cheb_rx && acgb200_cheb_step && acgb200_cheb_fused_step && acgb200_cheb_p;
+}
+
+static double *cheb_vec(const struct priv *pv, int i)     /* 0 D^-1, 1 z, 2 res, 3 d_0, 4 d_1 */
+{
+    return pv->d_cvec + (size_t) i * ((size_t) pv->nowned + 2);
+}
+
+/* the scalars and vectors, made once per solver, and D^-1 with its count of invalid diagonal entries */
+static int cheb_alloc(struct solvectx *c)
+{
+    struct acgsolvercuda *cg = c->cg;
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    if (!pv->d_cs) {
+        CU(cudaMalloc((void **) &pv->d_cs, sizeof(*pv->d_cs)));
+        CU(cudaMallocHost((void **) &pv->h_cs, sizeof(*pv->h_cs)));
+        pv->cheb_baddiag = -1;
+    }
+    if (!pv->d_cvec) {
+        const size_t bytes = 5 * ((size_t) pv->nowned + 2) * sizeof(double);
+        CU(cudaMalloc((void **) &pv->d_cvec, bytes));
+        CU(cudaMemset(pv->d_cvec, 0, bytes));
+    }
+    if (pv->cheb_baddiag < 0) {
+        struct acgb200_cstate cs;
+        memset(&cs, 0, sizeof(cs));
+        OK(scalars_push(c, pv->d_cs, pv->h_cs, &cs, sizeof(cs)));
+        KL(acgb200_cheb_dinv(pv->nowned, cg->d_rowptr, cg->d_colidx, cg->d_a, cheb_vec(pv, 0), pv->d_cs, pv->stream));
+        OK(scalars_pull(c, pv->d_cs, pv->h_cs, &cs, sizeof(cs)));
+        pv->cheb_baddiag = cs.baddiag;
+    }
+    return ACG_SUCCESS;
+}
+
+/* r0 = b - A x into d_r with (r0,r0) folded in */
+static int cheb_residual(struct solvectx *c, double *rr)
+{
+    struct priv *pv = c->pv;
+    struct acgb200_devstate h;
+    memset(&h, 0, sizeof(h));
+    OK(scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h)));
+    *rr = 0;
+    OK(apply_A(c, c->d_x, c->d_x, c->cg->d_r, c->d_b, SPMV_R_B_AX, &pv->d_st->tmp_loc[0], 0, 0, 0, -1));
+    return reduce_to_host(c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, rr);
+}
+
+/* the start c0 = 1/theta and the steps' (rho_j rho_{j-1}, 2 rho_j / delta) of the interval [a, b] (Saad,
+ * Iterative Methods, Alg. 12.1; tests/chebref.py coefficients) */
+static void cheb_coefficients(struct solvectx *c, double a, double b)
+{
+    const double theta = (a + b) / 2, delta = (b - a) / 2, sigma = theta / delta;
+    double rho = 1 / sigma;
+    c->cheb_c0 = 1 / theta;
+    for (int j = 0; j < c->cheb_degree; j++) {
+        const double rn = 1 / (2 * sigma - rho);
+        c->cheb_c[j][0] = rn * rho; c->cheb_c[j][1] = 2 * rn / delta;
+        rho = rn;
+    }
+}
+
+/* the d inner steps of z = M^-1 r after the r/x kernel: d_{j-1} in buffer (j-1)&1, d_j into the other */
+static int cheb_steps(struct solvectx *c)
+{
+    struct acgsolvercuda *cg = c->cg;
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    const int n = pv->nowned;
+    for (int j = 1; j <= c->cheb_degree; j++) {
+        const double *dprev = cheb_vec(pv, 3 + ((j - 1) & 1));
+        double *dnext = cheb_vec(pv, 3 + (j & 1));
+        const int last = j == c->cheb_degree;
+        const double c1 = c->cheb_c[j - 1][0], c2 = c->cheb_c[j - 1][1];
+        if (c->cheb_fused) {
+            struct acgb200_chebargs a;
+            memset(&a, 0, sizeof(a));
+            a.plan = &pv->plan; a.rowptr = cg->d_rowptr; a.colidx = cg->d_colidx; a.a = cg->d_a;
+            a.st = pv->d_st; a.cs = pv->d_cs; a.c1 = c1; a.c2 = c2; a.last = last;
+            a.q = cg->d_t; a.dinv = cheb_vec(pv, 0); a.dprev = dprev; a.dnext = dnext;
+            a.res = cheb_vec(pv, 2); a.z = cheb_vec(pv, 1); a.r = c->cheb_r;
+            KL(acgb200_cheb_fused_step(&a, pv->stream));
+            c->launches += 1 + (pv->plan.ntiles > 0);
+        } else {
+            /* the plan's product into t (consumed by the r/x kernel already), gated by ctrl[2] */
+            OK(apply_A(c, dprev, (double *) dprev, cg->d_t, NULL, SPMV_Y_AX, NULL, 2, 0, 0, -1));
+            KL(acgb200_cheb_step(n, pv->d_st, pv->d_cs, c1, c2, last, cg->d_t, cheb_vec(pv, 0), dprev, dnext,
+                                 cheb_vec(pv, 2), cheb_vec(pv, 1), c->cheb_r, pv->stream));
+            c->launches += 1;
+        }
+    }
+    return ACG_SUCCESS;
+}
+
+/* The set-up of a loop of c->cheb_degree from c->cheb_r: zeroed scalars, z_0 = M^-1 r_0 with (r_0, z_0) into rz
+ * slot 0 (the preconditioner of "iteration -1": the r/x kernel's start and the inner steps, under a word with
+ * iteration -1), p_0 = z_0, then the control words of iteration 0 */
+static int cheb_start(struct solvectx *c, int maxits, double tol, int log)
+{
+    struct acgsolvercuda *cg = c->cg;
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    const int n = pv->nowned;
+    struct acgb200_cstate cs;
+    memset(&cs, 0, sizeof(cs));
+    cs.log = log;
+    OK(scalars_push(c, pv->d_cs, pv->h_cs, &cs, sizeof(cs)));
+    struct acgb200_devstate h;
+    memset(&h, 0, sizeof(h));
+    h.maxits = maxits; h.tol = tol;
+    h.ctrl[1].iter = h.ctrl[2].iter = -1;
+    OK(scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h)));
+    KL(acgb200_cheb_rx(n, pv->d_st, pv->d_cs, 1, c->cheb_degree > 0, c->cheb_c0, cheb_vec(pv, 0), NULL, NULL, NULL,
+                       c->cheb_r, cheb_vec(pv, 1), cheb_vec(pv, 2), cheb_vec(pv, 3), pv->stream));
+    c->launches += 1;
+    OK(cheb_steps(c));
+    CU(cudaMemcpyAsync(cg->d_p, cheb_vec(pv, 1), (size_t) n * sizeof(double), cudaMemcpyDeviceToDevice, pv->stream));
+    h.ctrl[1].iter = h.ctrl[2].iter = 0;
+    return scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h));
+}
+
+/* iteration k: t = A p (+ (p, t)), the r/x kernel, the d inner steps, the p kernel */
+static int cheb_iteration(struct solvectx *c, int k)
+{
+    struct acgsolvercuda *cg = c->cg;
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    const int n = pv->nowned;
+    OK(apply_A(c, cg->d_p, cg->d_p, cg->d_t, NULL, SPMV_Y_AX_DOT, &pv->d_cs->pap[k & 1], 1, 0, 0, 0));
+    prof_mark(c, &pv->blas);
+    KL(acgb200_cheb_rx(n, pv->d_st, pv->d_cs, 0, c->cheb_degree > 0, c->cheb_c0, cheb_vec(pv, 0), cg->d_t, cg->d_p,
+                       c->cheb_x, c->cheb_r, cheb_vec(pv, 1), cheb_vec(pv, 2), cheb_vec(pv, 3), pv->stream));
+    OK(cheb_steps(c));
+    KL(acgb200_cheb_p(n, pv->d_st, pv->d_cs, cheb_vec(pv, 1), cg->d_p, pv->stream));
+    prof_mark(c, &pv->blas);
+    c->launches += 2;
+    return ACG_SUCCESS;
+}
+
+/* eigenvalues of the symmetric tridiagonal (diagonal a, off-diagonal e) below x: the negative pivots of
+ * T - x I = L D L^T (Sturm count; a zero pivot counts as negative) */
+static int sturm_count(int k, const double *a, const double *e, double x)
+{
+    int cnt = 0;
+    double q = 1.0;
+    for (int j = 0; j < k; j++) {
+        q = a[j] - x - (j > 0 ? e[j - 1] * e[j - 1] / q : 0.0);
+        if (q == 0.0) q = -DBL_MIN;
+        if (q < 0.0) cnt++;
+    }
+    return cnt;
+}
+
+/* eigenvalue i (ascending) of the tridiagonal by bisection of the Gershgorin interval [lo, hi] */
+static double sturm_eigenvalue(int k, const double *a, const double *e, int i, double lo, double hi)
+{
+    for (int it = 0; it < 2200; it++) {
+        const double mid = 0.5 * (lo + hi);
+        if (mid <= lo || mid >= hi) break;
+        if (sturm_count(k, a, e, mid) > i) hi = mid;
+        else lo = mid;
+    }
+    return 0.5 * (lo + hi);
+}
+
+int acgb200_cheb_interval_host(int k, const double *alpha, const double *beta, double *theta_min, double *theta_max)
+{
+    if (k < 1 || !alpha || (k > 1 && !beta) || !theta_min || !theta_max) return ACG_ERR_INVALID_VALUE;
+    for (int j = 0; j < k; j++) {
+        if (!(alpha[j] > 0 && isfinite(alpha[j]))) return ACG_ERR_INVALID_VALUE;
+        if (j + 1 < k && !(beta[j] >= 0 && isfinite(beta[j]))) return ACG_ERR_INVALID_VALUE;
+    }
+    double *a = malloc(2 * (size_t) k * sizeof(double));
+    if (!a) return ACG_ERR_ERRNO;
+    double *e = a + k;
+    /* the Lanczos matrix of k CG steps: 1/alpha_j + beta_{j-1}/alpha_{j-1} on the diagonal, sqrt(beta_j)/alpha_j
+     * beside it */
+    double lo = INFINITY, hi = -INFINITY;
+    for (int j = 0; j < k; j++) {
+        a[j] = 1 / alpha[j] + (j > 0 ? beta[j - 1] / alpha[j - 1] : 0.0);
+        if (j + 1 < k) e[j] = sqrt(beta[j]) / alpha[j];
+    }
+    for (int j = 0; j < k; j++) {
+        const double rad = (j > 0 ? e[j - 1] : 0.0) + (j + 1 < k ? e[j] : 0.0);
+        if (a[j] - rad < lo) lo = a[j] - rad;
+        if (a[j] + rad > hi) hi = a[j] + rad;
+    }
+    const double pad = 4 * DBL_EPSILON * fmax(fabs(lo), fabs(hi)) + DBL_MIN;
+    lo -= pad; hi += pad;
+    *theta_min = sturm_eigenvalue(k, a, e, 0, lo, hi);
+    *theta_max = sturm_eigenvalue(k, a, e, k - 1, lo, hi);
+    free(a);
+    return ACG_SUCCESS;
+}
+
+/* The upper bound's estimate: ACGB200_CHEB_EST Jacobi-PCG steps from r0 (in d_r) on scratch vectors -- r in
+ * res, p and t in d_p and d_t, z in z, x not updated -- with their alpha and beta logged, stopping early on
+ * ||r|| < tol or a breakdown; *steps of them ran, and theta_max is the largest eigenvalue of their Lanczos
+ * matrix (0 if none ran). */
+static int cheb_estimate(struct solvectx *c, double tol, int *steps, double *theta_max)
+{
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    const int degree = c->cheb_degree, fused = c->cheb_fused;
+    double *const r = c->cheb_r, *const x = c->cheb_x;
+    c->cheb_degree = 0; c->cheb_fused = 0;
+    c->cheb_r = cheb_vec(pv, 2); c->cheb_x = NULL;
+    CU(cudaMemcpyAsync(c->cheb_r, c->cg->d_r, (size_t) pv->nowned * sizeof(double), cudaMemcpyDeviceToDevice,
+                       pv->stream));
+    OK(cheb_start(c, ACGB200_CHEB_EST, tol, 1));
+    for (int i = 0; i < ACGB200_CHEB_EST; i++) OK(cheb_iteration(c, i));
+    struct acgb200_devstate h;
+    struct acgb200_cstate cs;
+    OK(scalars_pull(c, pv->d_st, pv->h_st, &h, sizeof(h)));
+    OK(scalars_pull(c, pv->d_cs, pv->h_cs, &cs, sizeof(cs)));
+    c->cheb_degree = degree; c->cheb_fused = fused; c->cheb_r = r; c->cheb_x = x;
+    *steps = h.ctrl[0].iter;
+    *theta_max = 0;
+    double tmin = 0;
+    if (*steps > 0) OK(acgb200_cheb_interval_host(*steps, cs.alpha_log, cs.beta_log, &tmin, theta_max));
+    return ACG_SUCCESS;
+}
+
+static void account_cheb(struct acgsolvercuda *cg, const struct priv *pv, int nits, int degree, int fused,
+                         int nsetup)
+{
+    /* Products: 1 + d per iteration and the set-up's (nsetup: the estimate's steps and the d steps of z_0), in the
+     * CSR model of account_classic.  Vector bytes per row: the r/x kernel 64 at degree 0 (p, t, x, r, D^-1
+     * read; x, r, z written) and 80 above it (res and d_0 written too); each inner step 56 (res, d_{j-1},
+     * D^-1, z read; res, d_j, z written), the last 48 (r read, z written only), and 8 more without fusion (the
+     * product's result read back); the p kernel 24 (z, p read; p written). */
+    const int64_t n = pv->nowned, nnz = pv->fnnz + pv->onnz;
+    const int64_t bgemv = nnz * 12 + n * 16 + (int64_t) pv->nvec * 8;
+    const int64_t nprod = (int64_t) nits * (1 + degree) + nsetup;
+    cg->ngemv += nprod; cg->nflops += nprod * 3 * nnz; cg->Bgemv += nprod * bgemv;
+    cg->ndot += 2 * (int64_t) nits; cg->nflops += (int64_t) nits * 4 * n; cg->Bdot += (int64_t) nits * 16 * n;
+    cg->nnrm2 += nits; cg->nflops += (int64_t) nits * 2 * n; cg->Bnrm2 += (int64_t) nits * 8 * n;
+    const int64_t bstep = degree > 0 ? 56 * (int64_t) (degree - 1) + 48 + (fused ? 0 : 8 * (int64_t) degree) : 0;
+    const int64_t bvec = (degree > 0 ? 80 : 64) + bstep + 24;
+    cg->naxpy += (3 + 2 * (int64_t) degree) * nits; cg->nflops += (int64_t) nits * (6 + 5 * (int64_t) degree) * n;
+    cg->Baxpy += (int64_t) nits * bvec * n;
+}
+
+int acgsolvercuda_solve_chebyshev(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A,
+                                  const struct acgvector *b, struct acgvector *x, int degree,
+                                  double lmin, double lmax, int maxits, double residualatol,
+                                  double residualrtol, int warmup, int *errcode)
+{
+    int errcode_ = 0;
+    if (!errcode) errcode = &errcode_;
+    cfg_load();
+    struct priv *pv = priv_of(cg);
+    if (!pv || !A || !b || !x) return ACG_ERR_INVALID_VALUE;
+    if (!have_cheb_kernels() || !one_gpu(pv, A)) return ACG_ERR_NOT_SUPPORTED;
+    if (maxits < 0 || degree < 0 || degree > ACGB200_CHEB_MAXDEG) return ACG_ERR_INVALID_VALUE;
+    /* the interval: non-negative and finite (0: estimated), a given lower bound below a given upper one */
+    if (degree > 0 && (!(isfinite(lmin) && lmin >= 0) || !(isfinite(lmax) && lmax >= 0) ||
+                       (lmin > 0 && lmax > 0 && lmin >= lmax))) return ACG_ERR_INVALID_VALUE;
+    struct acgcomm null = null_comm();
+    struct solvectx c;
+    OK(solve_begin(&c, cg, A, b, x, 0.0, 0.0, &null, 0, errcode));
+    c.kind = KIND_CHEB;
+    const int n = pv->nowned;
+    OK(cheb_alloc(&c));
+    if (pv->cheb_baddiag != 0) return ACG_ERR_INVALID_VALUE;
+    c.cheb_degree = degree;
+    /* one kernel per inner step where the pipelined solve fuses its iteration: mirrored diagonals for the slice
+     * rows, all other rows in tiles (DESIGN.md sections 4a and 15) */
+    const struct acgb200_spmvplan *pl = &pv->plan;
+    c.cheb_fused = degree > 0 && pl->nslices > 0 && pl->symdiag_nd > 0 && pl->nmtiles == 0 && pl->nmed == 0
+                   && pl->nlong == 0;
+    c.cheb_r = cg->d_r; c.cheb_x = c.d_x;
+    struct acgb200_devstate h;
+
+    /* warm-up: the set-up and `warmup` iterations (any interval) on x itself, then x0 again from the caller's
+     * vector */
+    if (warmup > 0) {
+        double rr = 0;
+        OK(cheb_residual(&c, &rr));
+        if (rr > 0) {
+            cheb_coefficients(&c, 0.2, 2.0);
+            OK(cheb_start(&c, warmup, 0.0, 0));
+            for (int i = 0; i < warmup; i++) OK(cheb_iteration(&c, i));
+        }
+        OK(upload_x0(&c, x));
+    }
+    OK(window_open(&c, maxits, residualatol, residualrtol, 0, 0));
+    pv->last_cheb_degree = degree;
+
+    /* ||b|| ; r0 = b - A x0 */
+    memset(&h, 0, sizeof(h));
+    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+    double bb = 0, rr0 = 0;
+    KL(acgb200_dot(n, c.d_b, c.d_b, &pv->d_st->tmp_loc[0], pv->stream));
+    OK(reduce_to_host(&c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &bb));
+    c.launches += 1;
+    cg->bnrm2 = sqrt(bb);
+    OK(cheb_residual(&c, &rr0));
+    cg->rnrm2 = cg->r0nrm2 = sqrt(rr0);
+    cg->nnrm2 += 2; cg->nflops += 4 * (int64_t) n; cg->Bnrm2 += 8 * (int64_t) n; cg->ngemv++;
+    const double tol = threshold(residualatol, residualrtol, cg->r0nrm2);
+    const double rtol_scaled = residualrtol * cg->r0nrm2;
+    int converged = tol > 0 && cg->rnrm2 < tol;                    /* acg/cgcuda.c:836-842 */
+    int nsetup = 0;
+
+    /* ||r0|| = 0: x0 solves the system */
+    if (!converged && maxits > 0 && rr0 > 0) {
+        double a = 0, bnd = degree > 0 ? lmax : 0;
+        int est = 0, started = 1;
+        if (degree > 0) {
+            if (lmax == 0) {
+                double tmax = 0;
+                OK(cheb_estimate(&c, tol, &est, &tmax));
+                bnd = 1.1 * tmax;
+                nsetup += est;
+                pv->last_cheb_est = est;
+            }
+            if (est > 0 || lmax > 0) {
+                a = lmin > 0 ? lmin : bnd / 10;
+                if (!(isfinite(bnd) && a < bnd)) return ACG_ERR_INVALID_VALUE;
+                pv->last_cheb_lmin = a; pv->last_cheb_lmax = bnd;
+                cheb_coefficients(&c, a, bnd);
+            } else {
+                /* no estimate step ran: (p, A p) or (r, z) of Jacobi PCG from r0 broke down */
+                started = 0;
+                pv->last_cheb_breakdown = 1;
+            }
+        }
+        if (started) {
+            /* the coefficients are arguments of the replayed kernels: a graph of another interval is not reused */
+            if (pv->graph[KIND_CHEB] && (pv->cheb_graph_ab[0] != a || pv->cheb_graph_ab[1] != bnd)) {
+                cudaGraphExecDestroy(pv->graph[KIND_CHEB]);
+                pv->graph[KIND_CHEB] = NULL;
+            }
+            pv->cheb_graph_ab[0] = a; pv->cheb_graph_ab[1] = bnd;
+            OK(cheb_start(&c, maxits, tol, 0));
+            nsetup += degree;
+            OK(iterate(&c, maxits, 1, cheb_iteration));
+            struct acgb200_cstate cs;
+            OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+            OK(scalars_pull(&c, pv->d_cs, pv->h_cs, &cs, sizeof(cs)));
+            cg->niterations = h.ctrl[0].iter;
+            if (cg->niterations > 0) cg->rnrm2 = sqrt(h.final_rr);
+            pv->last_cheb_breakdown = cs.breakdown;
+        }
+        converged = tol > 0 && cg->rnrm2 < tol;
+        cg->ntotaliterations += cg->niterations;
+    }
+    OK(window_close(&c));
+    account_cheb(cg, pv, cg->niterations, degree, c.cheb_fused, nsetup);
+    return solve_end(&c, x, not_converged(converged, residualatol, rtol_scaled) ? ACG_ERR_NOT_CONVERGED : ACG_SUCCESS);
+}
+
+/* ------------------------------------------------------------------------ */
 /* pipelined CG                                                              */
 /* ------------------------------------------------------------------------ */
 
@@ -2805,5 +3182,8 @@ int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info
     info->spmv_symdiag_codes = pv->plan.symdiag_codes;
     info->spmv_symdiag_code_bytes = pv->plan.symdiag_codes > 0 ? (int64_t) pv->plan.symdiag_nd * pv->plan.symdiag_stride : 0;
     info->mixed_reliable_updates = pv->last_mixed_updates;
+    info->cheb_degree = pv->last_cheb_degree; info->cheb_est_iterations = pv->last_cheb_est;
+    info->cheb_breakdown = pv->last_cheb_breakdown;
+    info->cheb_lmin = pv->last_cheb_lmin; info->cheb_lmax = pv->last_cheb_lmax;
     return ACG_SUCCESS;
 }

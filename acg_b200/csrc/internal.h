@@ -585,6 +585,72 @@ ACGB200_MULTI_LAUNCHER int acgb200_mixed_replace(int n, struct acgb200_devstate 
 /* x += sigma y (the fold at maxits; ungated) */
 ACGB200_MULTI_LAUNCHER int acgb200_mixed_fold(int n, double sigma, const float *y, double *x, cudaStream_t stream);
 
+/* ------------------------------------------------------------------------
+ * Chebyshev-preconditioned CG (acgsolvercuda_solve_chebyshev): PCG with
+ * M^-1 = p_d(D^-1 A) D^-1, z = M^-1 r formed by d steps of Jacobi-scaled
+ * Chebyshev iteration on A z = r from z = 0 (DESIGN.md section 15).
+ * Iteration k (parity s = k&1) runs:
+ *   1. t = A p with (p, t) into pap[s]                        reads ctrl[0]
+ *   2. the r/x kernel: alpha = rz[k%3]/pap[s], x += alpha p, r -= alpha t,
+ *      (r, r) into rr[s], and the preconditioner's start (degree 0: z = D^-1 r
+ *      with (r, z) into rz[(k+1)%3])            reads ctrl[1], writes ctrl[2]
+ *   3. d inner steps res -= A d_{j-1}, d_j = c1_j d_{j-1} + c2_j D^-1 res,
+ *      z += d_j; the last adds (r, z) into rz[(k+1)%3]          read ctrl[2]
+ *   4. the p kernel: the test on (r, r), p = z + beta p      reads ctrl[2],
+ *      writes ctrl[0]
+ * (r, z) lives in a ring of three slots: the p kernel of iteration k reads
+ * slots k%3 and (k+1)%3 and zeroes (k+2)%3, so no kernel reads a slot it
+ * writes.  The set-up's preconditioner is that of "iteration -1": it adds into
+ * slot 0.
+ * ------------------------------------------------------------------------ */
+#define ACGB200_CHEB_MAXDEG 16
+#define ACGB200_CHEB_EST 10             /* Jacobi-PCG steps of the interval estimate */
+struct acgb200_cstate {
+    double pap[2];                   /* (p, A p) of iteration k in slot k&1 */
+    double rr[2];                    /* (r_{k+1}, r_{k+1}) of iteration k in slot k&1 */
+    double rz[3];                    /* (r_k, z_k) in slot k%3 */
+    double alpha_log[ACGB200_CHEB_EST], beta_log[ACGB200_CHEB_EST];   /* the estimate's alpha_k, beta_k */
+    int log;                         /* 1: log alpha_k and beta_k (the estimate) */
+    int breakdown;                   /* 1: (p, A p) or (r, z) <= 0 or non-finite ended the solve */
+    int baddiag;                     /* diagonal entries <= 0 or non-finite (acgb200_cheb_dinv) */
+    int pad;
+};
+/* dinv_i = 1 / a_ii of the full-storage local block; cs->baddiag += entries that are <= 0, non-finite or absent */
+ACGB200_MULTI_LAUNCHER int acgb200_cheb_dinv(int n, const int *rowptr, const int *colidx, const double *a, double *dinv,
+                                             struct acgb200_cstate *cs, cudaStream_t stream);
+/* step 2 (reads ctrl[1], writes ctrl[2]).  start: the set-up's preconditioner start only (no breakdown test,
+ * no update of x and r); x == NULL: x is not updated (the estimate).  cheb: res = r, d0 = c0 D^-1 r, z = d0;
+ * otherwise z = D^-1 r with (r, z) folded in. */
+ACGB200_MULTI_LAUNCHER int acgb200_cheb_rx(int n, struct acgb200_devstate *st, struct acgb200_cstate *cs, int start,
+                                           int cheb, double c0, const double *dinv, const double *t, const double *p,
+                                           double *x, double *r, double *z, double *res, double *d0,
+                                           cudaStream_t stream);
+/* step 3 on plans without the fused path: after q = A dprev, res -= q, dnext = c1 dprev + c2 D^-1 res,
+ * z += dnext; last: (r, z) folded in, res and dnext not stored (reads ctrl[2]) */
+ACGB200_MULTI_LAUNCHER int acgb200_cheb_step(int n, const struct acgb200_devstate *st, struct acgb200_cstate *cs, double c1,
+                                             double c2, int last, const double *q, const double *dinv,
+                                             const double *dprev, double *dnext, double *res, double *z,
+                                             const double *r, cudaStream_t stream);
+/* step 3 in one kernel per step (two with tiles) on plans with mirrored diagonals and no merge tiles, medium
+ * or long rows: the mirrored-diagonal product of dprev goes straight into the step; the tile rows' product
+ * goes to q first and is finished by the same kernel */
+struct acgb200_chebargs {
+    const struct acgb200_spmvplan *plan;
+    const int *rowptr, *colidx; const double *a;    /* CSR of the tile rows */
+    const struct acgb200_devstate *st;
+    struct acgb200_cstate *cs;
+    double c1, c2;
+    int last;
+    double *q;                                      /* the tile rows' product */
+    const double *dinv, *dprev;
+    double *dnext, *res, *z;
+    const double *r;
+};
+ACGB200_MULTI_LAUNCHER int acgb200_cheb_fused_step(const struct acgb200_chebargs *a, cudaStream_t stream);
+/* step 4 (reads ctrl[2], writes ctrl[0]) */
+ACGB200_MULTI_LAUNCHER int acgb200_cheb_p(int n, struct acgb200_devstate *st, struct acgb200_cstate *cs,
+                                          const double *z, double *p, cudaStream_t stream);
+
 /* setup-time helpers */
 int acgb200_dot(int n, const double *x, const double *y, double *acc, cudaStream_t stream); /* acc += x.y */
 int acgb200_dot2(int n, const double *r, const double *w, double *acc2, cudaStream_t stream); /* acc2[0]+=r.r, acc2[1]+=w.r */

@@ -840,6 +840,44 @@ template <typename X> __device__ __forceinline__ X *sd_vec(double *p) { return r
 __device__ __forceinline__ double sd_decode(double v, const double *) { return v; }
 __device__ __forceinline__ double sd_decode(unsigned c, const double *vtab_s) { return vtab_s[c]; }
 
+/* Row `row`'s sum of the mirrored-diagonal product: L entries in batches of UB value loads and UB gathers,
+ * one FMA chain in ascending offset.  tab_s and vtab_s are the kernel's shared copies of P.tab and P.vtab. */
+template <int UB, typename V, typename X>
+__device__ __forceinline__ double symdiag_row_sum(const SymdiagParams &P, const int2 *tab_s, const double *vtab_s, int row,
+                                                  uint64_t pol, int cmax, int L)
+{
+    constexpr bool CODED = std::is_same<V, uint8_t>::value;
+    typedef decltype(ld_stream((const V *) nullptr, 0)) R;      /* a loaded value or code */
+    const V *hv = (CODED ? (const V *) P.hcode : (const V *) P.hval) + row;
+    double sum = 0.0;
+    int e = 0;
+    for (; e + UB <= L; e += UB) {
+        R cv[UB];
+        double vv[UB], xv[UB];
+#pragma unroll
+        for (int u = 0; u < UB; u++) cv[u] = ld_stream(hv + tab_s[e + u].x, pol);
+#pragma unroll
+        for (int u = 0; u < UB; u++) xv[u] = ld_x(sd_vec<X>(P.x) + min(max(row + tab_s[e + u].y, 0), cmax));
+#pragma unroll
+        for (int u = 0; u < UB; u++) vv[u] = sd_decode(cv[u], vtab_s);
+        sum = slice_fma<UB>(vv, xv, sum);
+    }
+    if (e < L) {
+        /* last, partial batch: slots past L are neither loaded nor added */
+        R cv[UB];
+        double vv[UB], xv[UB];
+#pragma unroll
+        for (int u = 0; u < UB; u++) cv[u] = e + u < L ? ld_stream(hv + tab_s[e + u].x, pol) : (R) 0;
+#pragma unroll
+        for (int u = 0; u < UB; u++) xv[u] = e + u < L ? ld_x(sd_vec<X>(P.x) + min(max(row + tab_s[e + u].y, 0), cmax)) : 0.0;
+#pragma unroll
+        for (int u = 0; u < UB; u++) vv[u] = sd_decode(cv[u], vtab_s);
+#pragma unroll
+        for (int u = 0; u < UB; u++) if (e + u < L) sum = fma(vv[u], xv[u], sum);
+    }
+    return sum;
+}
+
 template <int UB, int T, bool PCG, typename V, typename X = double>
 __global__ void __launch_bounds__(T, PCG ? 1536 / T : 0)
 spmv_symdiag_kernel(const SymdiagParams P)
@@ -847,7 +885,6 @@ spmv_symdiag_kernel(const SymdiagParams P)
     constexpr bool CODED = std::is_same<V, uint8_t>::value;
     constexpr bool F32 = std::is_same<X, float>::value;
     static_assert(!(F32 && PCG), "the fused pipelined-CG epilogue is fp64 only");
-    typedef decltype(ld_stream((const V *) nullptr, 0)) R;      /* a loaded value or code */
     __shared__ int2 tab_s[ACGB200_SYMDIAG_MAX];
     __shared__ double vtab_s[CODED ? 256 : 1];
     __shared__ double red[T / 32];
@@ -893,33 +930,7 @@ spmv_symdiag_kernel(const SymdiagParams P)
     const uint64_t vpol = PCG ? (P.vec_evict_first ? l2_policy_evict_first() : l2_policy_evict_normal()) : 0;
     for (int s = warp; s < P.nslices; s += nwarps) {
         const int row = __ldg(&P.slices[s].row0) + lane;
-        const V *hv = (CODED ? (const V *) P.hcode : (const V *) P.hval) + row;
-        double sum = 0.0;
-        int e = 0;
-        for (; e + UB <= L; e += UB) {
-            R cv[UB];
-            double vv[UB], xv[UB];
-#pragma unroll
-            for (int u = 0; u < UB; u++) cv[u] = ld_stream(hv + tab_s[e + u].x, pol);
-#pragma unroll
-            for (int u = 0; u < UB; u++) xv[u] = ld_x(sd_vec<X>(P.x) + min(max(row + tab_s[e + u].y, 0), cmax));
-#pragma unroll
-            for (int u = 0; u < UB; u++) vv[u] = sd_decode(cv[u], vtab_s);
-            sum = slice_fma<UB>(vv, xv, sum);
-        }
-        if (e < L) {
-            /* last, partial batch: slots past L are neither loaded nor added */
-            R cv[UB];
-            double vv[UB], xv[UB];
-#pragma unroll
-            for (int u = 0; u < UB; u++) cv[u] = e + u < L ? ld_stream(hv + tab_s[e + u].x, pol) : (R) 0;
-#pragma unroll
-            for (int u = 0; u < UB; u++) xv[u] = e + u < L ? ld_x(sd_vec<X>(P.x) + min(max(row + tab_s[e + u].y, 0), cmax)) : 0.0;
-#pragma unroll
-            for (int u = 0; u < UB; u++) vv[u] = sd_decode(cv[u], vtab_s);
-#pragma unroll
-            for (int u = 0; u < UB; u++) if (e + u < L) sum = fma(vv[u], xv[u], sum);
-        }
+        const double sum = symdiag_row_sum<UB, V, X>(P, tab_s, vtab_s, row, pol, cmax, L);
         if (PCG) {
             /* w_i was gathered by this row a moment ago: an L1 hit, not a third stream */
             pcg_row(row, sum, __ldg(P.x + row), k, P.z, P.t, P.p, P.r, P.xs, P.w_next, vpol, dot, dot2);
@@ -2628,6 +2639,198 @@ mixed_fold_kernel(int n, double sigma, const float *__restrict__ y, double *__re
         x[i] = __dadd_rn(x[i], sigma * (double) y[i]);
 }
 
+/* ---- Chebyshev-preconditioned CG (DESIGN section 15) ----------------------------------------------- */
+
+/* dinv_i = 1 / a_ii, a_ii the sum of row i's diagonal entries in the full-storage block (0 if it has none);
+ * entries that are <= 0 or non-finite are counted into cs->baddiag */
+__global__ void __launch_bounds__(256)
+cheb_dinv_kernel(int n, const int *__restrict__ rowptr, const int *__restrict__ colidx, const double *__restrict__ a,
+                 double *__restrict__ dinv, acgb200_cstate *cs)
+{
+    int bad = 0;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        double v = 0.0;
+        for (int k = rowptr[i]; k < rowptr[i + 1]; k++) if (colidx[k] == i) v += a[k];
+        if (!(v > 0.0 && isfinite(v))) bad++;
+        dinv[i] = 1.0 / v;
+    }
+    if (bad) atomicAdd(&cs->baddiag, bad);
+}
+
+/* The r/x kernel of iteration k (reads ctrl[1], writes ctrl[2]): (p, A p) or (r_k, z_k) <= 0 or non-finite
+ * ends the solve before the update; otherwise alpha = (r_k, z_k) / (p, A p), x += alpha p (unless x is NULL),
+ * r -= alpha t with (r, r) into rr[s], and the preconditioner's start from the new r: with cheb, res = r,
+ * d0 = c0 (D^-1 r) and z = d0; without, z = D^-1 r with (r, z) into rz[(k+1)%3].  start: the set-up's
+ * preconditioner start from r as it is (the word's iteration is -1, so it adds into rz slot 0). */
+__global__ void __launch_bounds__(BLAS1_THREADS)
+cheb_rx_kernel(int n, acgb200_devstate *st, acgb200_cstate *cs, int start, int cheb, double c0,
+               const double *__restrict__ dinv, const double *__restrict__ t, const double *__restrict__ p,
+               double *__restrict__ x, double *__restrict__ r, double *__restrict__ z, double *__restrict__ res,
+               double *__restrict__ d0)
+{
+    __shared__ double red[BLAS1_THREADS / 32];
+    pdl_prologue();
+    const Gate g = gate_read(&st->ctrl[1], st);
+    const int s = g.iter & 1;
+    const double rz = start ? 1.0 : cs->rz[g.iter % 3], pap = start ? 1.0 : cs->pap[s];
+    const bool bad = !(rz > 0.0 && isfinite(rz)) || !(pap > 0.0 && isfinite(pap));
+    const double alpha = rz / pap;
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        acgb200_ctrl c = st->ctrl[1];
+        if (g.active && bad) { c.done = 1; cs->breakdown = 1; }
+        else if (g.active && !start && cs->log && g.iter < ACGB200_CHEB_EST) cs->alpha_log[g.iter] = alpha;
+        st->ctrl[2] = c;
+    }
+    if (!g.active || bad) return;
+    double rr = 0.0, rzn = 0.0;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        double ri = r[i];
+        if (!start) {
+            if (x) x[i] = fma(alpha, p[i], x[i]);
+            ri = fma(-alpha, t[i], ri);
+            r[i] = ri;
+            rr = fma(ri, ri, rr);
+        }
+        const double zi = dinv[i] * ri;
+        if (cheb) {
+            const double dv = c0 * zi;
+            res[i] = ri; d0[i] = dv; z[i] = dv;
+        } else {
+            z[i] = zi;
+            rzn = fma(ri, zi, rzn);
+        }
+    }
+    if (!start) {
+        rr = block_sum(rr, red);
+        if (threadIdx.x == 0) atomicAdd(&cs->rr[s], rr);
+    }
+    if (!cheb) {
+        rzn = block_sum(rzn, red);
+        if (threadIdx.x == 0) atomicAdd(&cs->rz[(g.iter + 1) % 3], rzn);
+    }
+}
+
+/* one row of a Chebyshev step, q_i = (A dprev)_i: res -= q, dnext = c1 dprev + c2 D^-1 res, z += dnext; the
+ * last step stores z only and adds r_i z_i into rz */
+__device__ __forceinline__ void cheb_row(int i, double qi, double c1, double c2, bool last, const double *__restrict__ dinv,
+                                         const double *__restrict__ dprev, double *__restrict__ dnext,
+                                         double *__restrict__ res, double *__restrict__ z, const double *__restrict__ r,
+                                         double &rz)
+{
+    const double rv = res[i] - qi;
+    const double dn = fma(c1, dprev[i], c2 * (dinv[i] * rv));
+    const double zv = z[i] + dn;
+    z[i] = zv;
+    if (last) rz = fma(r[i], zv, rz);
+    else { res[i] = rv; dnext[i] = dn; }
+}
+
+/* a Chebyshev step after the plan's ordinary product q = A dprev (reads ctrl[2]) */
+__global__ void __launch_bounds__(BLAS1_THREADS)
+cheb_step_kernel(int n, const acgb200_devstate *st, acgb200_cstate *cs, double c1, double c2, int last,
+                 const double *__restrict__ q, const double *__restrict__ dinv, const double *__restrict__ dprev,
+                 double *__restrict__ dnext, double *__restrict__ res, double *__restrict__ z,
+                 const double *__restrict__ r)
+{
+    __shared__ double red[BLAS1_THREADS / 32];
+    pdl_prologue();
+    const Gate g = gate_read(&st->ctrl[2], st);
+    if (!g.active) return;
+    double rz = 0.0;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        cheb_row(i, q[i], c1, c2, last, dinv, dprev, dnext, res, z, r, rz);
+    if (last) {
+        rz = block_sum(rz, red);
+        if (threadIdx.x == 0) atomicAdd(&cs->rz[(g.iter + 1) % 3], rz);
+    }
+}
+
+/* the Chebyshev step's part of the fused kernel's parameters; P.x of SymdiagParams is dprev */
+struct ChebStep {
+    const acgb200_tile *tiles;
+    int ntiles;
+    int last;
+    acgb200_cstate *cs;
+    double c1, c2;
+    const double *q, *dinv, *r;
+    double *dnext, *res, *z;
+};
+
+/*
+ * One Chebyshev step in one kernel: the mirrored-diagonal product of dprev (symdiag_row_sum, the row sums of
+ * spmv_symdiag_kernel bit for bit) goes straight into the row's step (cheb_row) instead of to memory.  Rows
+ * outside the slices -- the tiles -- take their product from q, written by the tile kernel just before; each
+ * CTA then finishes whole tiles.  dnext is another buffer than dprev: other rows still gather dprev.  The
+ * coefficients are arguments.  Reads ctrl[2] and writes no control word.  At most 40 registers: 12 CTAs of
+ * 128 threads, as the fused pipelined-CG kernel.
+ */
+template <int UB, int T, typename V>
+__global__ void __launch_bounds__(T, 1536 / T)
+spmv_symdiag_cheb_kernel(const SymdiagParams P, const ChebStep C)
+{
+    constexpr bool CODED = std::is_same<V, uint8_t>::value;
+    __shared__ int2 tab_s[ACGB200_SYMDIAG_MAX];
+    __shared__ double vtab_s[CODED ? 256 : 1];
+    __shared__ double red[T / 32];
+    const int tid = threadIdx.x;
+    pdl_prologue();
+    if (!gate_read(P.ctrl_in, P.st).active) return;
+    if (tid < P.no) tab_s[tid] = make_int2(P.tab[tid].voff, P.tab[tid].coff);
+    if (CODED) for (int i = tid; i < P.ncodes; i += T) vtab_s[i] = __ldg(P.vtab + i);
+    __syncthreads();
+    const uint64_t pol = P.evict_first ? l2_policy_evict_first() : l2_policy_evict_normal();
+    const int lane = tid & 31;
+    const int warp = (blockIdx.x * T + tid) >> 5;
+    const int nwarps = (gridDim.x * T) >> 5;
+    const int cmax = P.nrows - 1;
+    double rz = 0.0;
+    for (int s = warp; s < P.nslices; s += nwarps) {
+        const int row = __ldg(&P.slices[s].row0) + lane;
+        const double sum = symdiag_row_sum<UB, V, double>(P, tab_s, vtab_s, row, pol, cmax, P.no);
+        cheb_row(row, sum, C.c1, C.c2, C.last, C.dinv, P.x, C.dnext, C.res, C.z, C.r, rz);
+    }
+    for (int b = blockIdx.x; b < C.ntiles; b += gridDim.x) {
+        const acgb200_tile tl = C.tiles[b];
+        for (int i = tl.row_begin + tid; i < tl.row_begin + tl.nrows; i += T)
+            cheb_row(i, C.q[i], C.c1, C.c2, C.last, C.dinv, P.x, C.dnext, C.res, C.z, C.r, rz);
+    }
+    if (C.last) {
+        rz = block_sum(rz, red);
+        /* the iteration index read again rather than kept live through the loop (the word is not written
+         * during this kernel) */
+        if (tid == 0) atomicAdd(&C.cs->rz[(P.ctrl_in->iter + 1) % 3], rz);
+    }
+}
+
+/* The p kernel of iteration k (reads ctrl[2], writes ctrl[0]): the iteration is counted; ||r_{k+1}|| < tol
+ * (strict) ends the solve, otherwise beta = (r_{k+1}, z_{k+1}) / (r_k, z_k) and p = z + beta p.  Block 0 zeroes
+ * the next iteration's accumulators pap[s^1], rr[s^1] and rz[(k+2)%3]. */
+__global__ void __launch_bounds__(BLAS1_THREADS)
+cheb_p_kernel(int n, acgb200_devstate *st, acgb200_cstate *cs, const double *__restrict__ z, double *__restrict__ p)
+{
+    pdl_prologue();
+    const Gate g = gate_read(&st->ctrl[2], st);
+    const int s = g.iter & 1;
+    const double rr = cs->rr[s];
+    const bool conv = st->tol > 0.0 && sqrt(rr) < st->tol;
+    const double beta = cs->rz[(g.iter + 1) % 3] / cs->rz[g.iter % 3];
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        acgb200_ctrl c = st->ctrl[2];
+        if (g.active) {
+            c.iter = g.iter + 1;
+            st->final_rr = rr;
+            if (conv) c.done = 1;
+            if (cs->log && g.iter < ACGB200_CHEB_EST) cs->beta_log[g.iter] = beta;
+            cs->pap[s ^ 1] = 0.0;
+            cs->rr[s ^ 1] = 0.0;
+            cs->rz[(g.iter + 2) % 3] = 0.0;
+        }
+        st->ctrl[0] = c;
+    }
+    if (!g.active || conv) return;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) p[i] = fma(beta, p[i], z[i]);
+}
+
 /* ------------------------------------------------------------------------ */
 /* host-side launchers (C linkage)                                           */
 /* ------------------------------------------------------------------------ */
@@ -2757,6 +2960,20 @@ static symdiag_fn symdiag_f32_variant(const acgb200_spmvplan *pl)
     const bool coded = pl->symdiag_codes > 0;
 #define X(u, t) if (UB == u && T == t) \
         return coded ? spmv_symdiag_kernel<u, t, false, uint8_t, float> : spmv_symdiag_kernel<u, t, false, double, float>;
+    X(5, 128) X(7, 128) X(8, 128) X(9, 128) X(7, 256) X(8, 256) X(9, 256)
+#undef X
+    return NULL;
+}
+
+typedef void (*symdiag_cheb_fn)(const SymdiagParams, const ChebStep);
+
+/* the fused Chebyshev step, for the same (UB, T) pairs */
+static symdiag_cheb_fn symdiag_cheb_variant(const acgb200_spmvplan *pl)
+{
+    const int UB = pl->slice_ub, T = pl->slice_threads;
+    const bool coded = pl->symdiag_codes > 0;
+#define X(u, t) if (UB == u && T == t) \
+        return coded ? spmv_symdiag_cheb_kernel<u, t, uint8_t> : spmv_symdiag_cheb_kernel<u, t, double>;
     X(5, 128) X(7, 128) X(8, 128) X(9, 128) X(7, 256) X(8, 256) X(9, 256)
 #undef X
     return NULL;
@@ -3343,6 +3560,77 @@ extern "C" int acgb200_mixed_fold(int n, double sigma, const float *y, double *x
     static int occ = 0;
     mixed_fold_kernel<<<blas1_grid(n, (const void *) mixed_fold_kernel, &occ), BLAS1_THREADS, 0, stream>>>(n, sigma, y, x);
     return (int) cudaGetLastError();
+}
+
+extern "C" int acgb200_cheb_dinv(int n, const int *rowptr, const int *colidx, const double *a, double *dinv,
+                                 acgb200_cstate *cs, cudaStream_t stream)
+{
+    if (n <= 0) return 0;
+    long long grid = ((long long) n + 255) / 256;
+    const long long cap = (long long) acgb200_num_sms() * 8;
+    if (grid > cap) grid = cap;
+    cheb_dinv_kernel<<<(int) grid, 256, 0, stream>>>(n, rowptr, colidx, a, dinv, cs);
+    return (int) cudaGetLastError();
+}
+
+extern "C" int acgb200_cheb_rx(int n, acgb200_devstate *st, acgb200_cstate *cs, int start, int cheb, double c0,
+                               const double *dinv, const double *t, const double *p, double *x, double *r, double *z,
+                               double *res, double *d0, cudaStream_t stream)
+{
+    static int occ = 0;
+    return (int) launch_chain(cheb_rx_kernel, blas1_grid(n, (const void *) cheb_rx_kernel, &occ), BLAS1_THREADS, 0,
+                              stream, n, st, cs, start, cheb, c0, dinv, t, p, x, r, z, res, d0);
+}
+
+extern "C" int acgb200_cheb_step(int n, const acgb200_devstate *st, acgb200_cstate *cs, double c1, double c2, int last,
+                                 const double *q, const double *dinv, const double *dprev, double *dnext, double *res,
+                                 double *z, const double *r, cudaStream_t stream)
+{
+    static int occ = 0;
+    return (int) launch_chain(cheb_step_kernel, blas1_grid(n, (const void *) cheb_step_kernel, &occ), BLAS1_THREADS, 0,
+                              stream, n, st, cs, c1, c2, last, q, dinv, dprev, dnext, res, z, r);
+}
+
+extern "C" int acgb200_cheb_fused_step(const acgb200_chebargs *a, cudaStream_t stream)
+{
+    const acgb200_spmvplan *pl = a->plan;
+    const symdiag_cheb_fn fn = symdiag_cheb_variant(pl);
+    if (!fn || pl->nslices <= 0 || pl->symdiag_nd <= 0 || pl->nmtiles > 0 || pl->nmed > 0 || pl->nlong > 0)
+        return (int) cudaErrorInvalidConfiguration;
+    acgb200_devstate *st = const_cast<acgb200_devstate *>(a->st);
+    if (pl->ntiles > 0) {
+        /* rows outside the slices: q = A dprev over the tiles (its copy of the word goes to ctrl[3], read by nobody) */
+        acgb200_spmvargs s;
+        memset(&s, 0, sizeof(s));
+        s.plan = pl; s.rowptr = a->rowptr; s.colidx = a->colidx; s.a = a->a; s.x = a->dprev; s.y = a->q;
+        s.mode = SPMV_Y_AX; s.ctrl_in = &st->ctrl[2]; s.ctrl_out = &st->ctrl[3]; s.st = st;
+        const int err = launch_tiles(&s, stream);
+        if (err) return err;
+    }
+    int per_sm = 0;
+    const cudaError_t oe = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void *) fn, pl->slice_threads, 0);
+    if (oe) return (int) oe;
+    SymdiagParams S;
+    memset(&S, 0, sizeof(S));
+    symdiag_params(pl, S);
+    S.x = a->dprev; S.mode = SPMV_Y_AX; S.ctrl_in = &st->ctrl[2]; S.st = st;
+    ChebStep C;
+    C.tiles = pl->d_tiles; C.ntiles = pl->ntiles; C.last = a->last; C.cs = a->cs; C.c1 = a->c1; C.c2 = a->c2;
+    C.q = a->q; C.dinv = a->dinv; C.r = a->r; C.dnext = a->dnext; C.res = a->res; C.z = a->z;
+    /* the product's grid (its L2 cap included), unless the registers allow fewer CTAs */
+    const long long fgrid = (long long) acgb200_num_sms() * (per_sm < 1 ? 1 : per_sm);
+    const int grid = (int) (fgrid < pl->slice_grid ? fgrid : pl->slice_grid);
+    const cudaError_t le = launch_chain(fn, grid, pl->slice_threads, (size_t) 0, stream, S, C);
+    if (le) return (int) le;
+    return (int) cudaGetLastError();
+}
+
+extern "C" int acgb200_cheb_p(int n, acgb200_devstate *st, acgb200_cstate *cs, const double *z, double *p,
+                              cudaStream_t stream)
+{
+    static int occ = 0;
+    return (int) launch_chain(cheb_p_kernel, blas1_grid(n, (const void *) cheb_p_kernel, &occ), BLAS1_THREADS, 0,
+                              stream, n, st, cs, z, p);
 }
 
 extern "C" int acgb200_gather(int n, double *dst, const double *src, const int *idx, cudaStream_t stream)

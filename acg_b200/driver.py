@@ -24,7 +24,8 @@ import numpy as np
 
 SOLVERS = {"acg": "solvempi", "acg-pipelined": "solve_pipelined",
            "acg-device": "solve_device", "acg-device-pipelined": "solve_device_pipelined",
-           "minres": "solve_minres", "mixed": "solve_mixed"}
+           "minres": "solve_minres", "mixed": "solve_mixed", "chebyshev": "solve_chebyshev"}
+ONE_PROCESS = ("minres", "mixed", "chebyshev")
 
 
 def parse_args(argv=None):
@@ -34,7 +35,9 @@ def parse_args(argv=None):
     ap.add_argument("--solver", default="acg", choices=sorted(SOLVERS),
                     help="minres: MINRES for symmetric indefinite or singular A, e.g. with a negative --epsilon "
                          "(acgsolvercuda_solve_minres; one process only); mixed: CG with float vectors and "
-                         "reliable updates to an fp64 tolerance (acgsolvercuda_solve_mixed; one process only)")
+                         "reliable updates to an fp64 tolerance (acgsolvercuda_solve_mixed; one process only); chebyshev: CG "
+                         "preconditioned with a Chebyshev polynomial in D^-1 A of --degree "
+                         "(acgsolvercuda_solve_chebyshev; one process only)")
     ap.add_argument("--max-iterations", type=int, default=100)
     ap.add_argument("--residual-atol", type=float, default=0.0)
     ap.add_argument("--residual-rtol", type=float, default=1e-9)
@@ -52,6 +55,11 @@ def parse_args(argv=None):
     ap.add_argument("--shifts", default=None, metavar="S0,S1,...",
                     help="solve (A + s_j I) x_j = b for 1-8 comma-separated shifts s_j >= 0 at once from x0 = 0: one CG "
                          "on A drives every shifted system (acgsolvercuda_solve_shifted; one process, classic solver)")
+    ap.add_argument("--degree", type=int, default=2,
+                    help="--solver chebyshev: the polynomial's degree, 0-16 (0: Jacobi)")
+    ap.add_argument("--interval", default=None, metavar="A,B",
+                    help="--solver chebyshev: the interval [A, B] of D^-1 A's spectrum (default: B estimated from 10 "
+                         "Jacobi-PCG steps, A = B/10)")
     ap.add_argument("--seed", type=int, default=1)
     ap.add_argument("--output-comm-matrix", metavar="PATH", help="write the halo send-count matrix (cuda/acg-cuda.c:1713-1775)")
     ap.add_argument("--output-solution", metavar="PATH", help="write x as a Matrix Market vector (text)")
@@ -176,7 +184,8 @@ def solve_shifted(args, A, cg, log):
 
 
 def solve_minres(args, A, cg, log):
-    """The --solver minres and --solver mixed runs: one solve_minres or solve_mixed call, the solver report,
+    """The --solver minres, mixed and chebyshev runs: one solve_minres, solve_mixed or solve_chebyshev call, the
+    solver report,
     then the iterations (and reliable updates), the solver's residual norm -- MINRES's recursively updated
     one, the mixed solve's fp64 one -- and the true residual ||b - A x|| (and the error norms with
     --manufactured-solution)."""
@@ -185,16 +194,28 @@ def solve_minres(args, A, cg, log):
     b = A.vector(); x = A.vector()
     b.x[:] = 0.0
     b.x[:n] = bo
-    code = getattr(cg, SOLVERS[args.solver])(b, x, maxits=args.max_iterations, residualatol=args.residual_atol,
-                                             residualrtol=args.residual_rtol, warmup=args.warmup)
+    kw = dict(maxits=args.max_iterations, residualatol=args.residual_atol, residualrtol=args.residual_rtol,
+              warmup=args.warmup)
+    if args.solver == "chebyshev":
+        lmin, lmax = args.interval or (0.0, 0.0)
+        kw.update(degree=args.degree, lmin=lmin, lmax=lmax)
+    code = getattr(cg, SOLVERS[args.solver])(b, x, **kw)
     log(cg.report())
     import scipy.sparse as sp
     rp = A.frowptr[:n + 1]
     F = sp.csr_matrix((A.fa[:rp[n]], A.fcolidx[:rp[n]] - A.c.rowidxbase, rp), shape=(n, n))
     true = float(np.linalg.norm(bo - F @ x.x[:n]))
-    upd = f" reliable updates {cg.info()['mixed_reliable_updates']}" if args.solver == "mixed" else ""
-    log(f"{args.solver}: iterations {cg.c.niterations}{upd} residual 2-norm {cg.c.rnrm2:.15g} "
-        f"true residual 2-norm {true:.15g} relative {true / cg.c.bnrm2 if cg.c.bnrm2 else 0.0:.3e}")
+    inf = cg.info()
+    upd = f" reliable updates {inf['mixed_reliable_updates']}" if args.solver == "mixed" else ""
+    if args.solver == "chebyshev":
+        how = "given" if args.interval else f"estimated from {inf['cheb_est_iterations']} steps"
+        upd = (f" degree {args.degree} interval [{inf['cheb_lmin']:.6g}, {inf['cheb_lmax']:.6g}] ({how})"
+               f" iterations {cg.c.niterations} products {cg.c.ngemv}")
+        log(f"chebyshev:{upd} residual 2-norm {cg.c.rnrm2:.15g} true residual 2-norm {true:.15g} "
+            f"relative {true / cg.c.bnrm2 if cg.c.bnrm2 else 0.0:.3e}")
+    else:
+        log(f"{args.solver}: iterations {cg.c.niterations}{upd} residual 2-norm {cg.c.rnrm2:.15g} "
+            f"true residual 2-norm {true:.15g} relative {true / cg.c.bnrm2 if cg.c.bnrm2 else 0.0:.3e}")
     if xstar is not None:
         log(f"initial error 2-norm: {np.linalg.norm(xstar):.15g}")
         log(f"error 2-norm: {np.linalg.norm(x.x[:n] - xstar):.15g}")
@@ -218,7 +239,19 @@ def main(argv=None):
     from . import dist as abdist, mtxio
     from .api import SolverCuda, SymCsrMatrix, mtx_info
 
-    if args.solver in ("minres", "mixed"):
+    if args.solver == "chebyshev":
+        if not 0 <= args.degree <= 16:
+            raise SystemExit("--degree must be between 0 and 16")
+        if args.interval is not None:
+            try:
+                args.interval = tuple(float(t) for t in args.interval.split(","))
+            except ValueError:
+                args.interval = ()
+            if len(args.interval) != 2 or not 0 < args.interval[0] < args.interval[1]:
+                raise SystemExit("--interval must be A,B with 0 < A < B")
+    elif args.interval is not None:
+        raise SystemExit("--interval and --degree belong to --solver chebyshev")
+    if args.solver in ONE_PROCESS:
         if int(os.environ.get("WORLD_SIZE", "1")) > 1:
             raise SystemExit(f"--solver {args.solver} runs in one process (one GPU, the whole matrix)")
         if args.nrhs is not None or args.shifts is not None:
@@ -292,7 +325,7 @@ def main(argv=None):
         cg.free()
         comm.destroy()
         return 0 if code == 0 else 1
-    if args.solver in ("minres", "mixed"):
+    if args.solver in ONE_PROCESS:
         code = solve_minres(args, A, cg, log)
         cg.free()
         comm.destroy()

@@ -145,6 +145,46 @@ ACG_API int acgsolvercuda_solve_mixed(struct acgsolvercuda *cg, const struct acg
  * poisoned on the device first.  One GPU, unpartitioned matrix.  For tests of the fp32 product. */
 ACG_API int acgsolvercuda_spmv_f32(struct acgsolvercuda *cg, const float *x, float *y, double *dot);
 
+/* A x = b for symmetric positive definite A by preconditioned CG with M^-1 = p_d(D^-1 A) D^-1 (one GPU).
+ *
+ * D is the diagonal of the operator the solver holds (the eps of acgsymcsrmatrix_dsymv_init included).
+ * z = M^-1 r is formed by d = `degree` steps of Jacobi-scaled Chebyshev iteration on A z = r from z = 0 over
+ * the interval [a, b] (Saad, Iterative Methods for Sparse Linear Systems, Alg. 12.1): theta = (a+b)/2,
+ * delta = (b-a)/2, sigma = theta/delta, rho_0 = 1/sigma; start res = r, d_0 = D^-1 r / theta, z = d_0; step
+ * j = 1..d: res -= A d_{j-1}, rho_j = 1/(2 sigma - rho_{j-1}), d_j = rho_j rho_{j-1} d_{j-1} +
+ * (2 rho_j/delta) D^-1 res, z += d_j.  M^-1 is symmetric positive definite exactly when every eigenvalue of
+ * D^-1 A lies in (0, a + b), so an underestimated upper bound still gives a valid preconditioner unless it is
+ * off by more than a.  degree = 0 is Jacobi PCG (z = D^-1 r); the interval is then ignored and nothing is
+ * estimated.  degree outside [0, 16] gives ACG_ERR_INVALID_VALUE.
+ *
+ * Interval: lmax = 0 estimates b = 1.1 theta_max, theta_max the largest eigenvalue of the Lanczos tridiagonal
+ * of 10 Jacobi-PCG steps from r0 on scratch vectors (fewer if the Krylov space breaks down or ||r|| < tol
+ * sooner; x and b are not touched).  lmin = 0 sets a = b/10.  A negative or non-finite bound, or a given lmin
+ * not below the given or estimated lmax, gives ACG_ERR_INVALID_VALUE before any iteration.
+ *
+ * Stopping as acgsolvercuda_solvempi: tol = threshold(atol, rtol, ||r0||) and the strict test ||r|| < tol on
+ * the recursively updated residual; ||r0|| < tol or ||r0|| = 0 runs no iteration; ACG_ERR_NOT_CONVERGED
+ * follows acgsolvercuda_solvempi's rule; maxits = 0 returns x0 unchanged.  (p, A p) <= 0, (r, z) <= 0 or
+ * either non-finite ends the solve before that iteration's update, which is not counted.  A diagonal entry
+ * that is <= 0 or non-finite gives ACG_ERR_INVALID_VALUE at set-up.  One GPU, unpartitioned matrix: ghost
+ * rows or more than one rank give ACG_ERR_NOT_SUPPORTED.  `warmup` iterations run first on scratch state;
+ * the results do not depend on them.
+ *
+ * niterations counts outer iterations (the estimate's steps not included); bnrm2, r0nrm2 and rnrm2 are set
+ * as by any solve; the counters count 1 + d products per iteration plus the set-up's and the estimate's.
+ * acgb200_info reports the degree, the estimate's steps, a breakdown and the interval used. */
+ACG_API int acgsolvercuda_solve_chebyshev(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A,
+                                          const struct acgvector *b, struct acgvector *x, int degree,
+                                          double lmin, double lmax, int maxits, double residualatol,
+                                          double residualrtol, int warmup, int *errcode);
+
+/* The extreme eigenvalues theta_min <= theta_max of the k x k Lanczos tridiagonal of k CG steps, as
+ * acgsolvercuda_solve_chebyshev builds it from its estimate's alpha_j (k of them, > 0) and beta_j (k - 1,
+ * >= 0): diagonal 1/alpha_j + beta_{j-1}/alpha_{j-1}, off-diagonal sqrt(beta_j)/alpha_j; Sturm bisection.
+ * For tests of the estimate. */
+ACG_API int acgb200_cheb_interval_host(int k, const double *alpha, const double *beta, double *theta_min,
+                                       double *theta_max);
+
 struct acgb200_info {
     int spmv_lanes_per_row, spmv_rows_cap, spmv_nnz_cap, spmv_stages;
     int spmv_ntiles, spmv_nlong, spmv_grid, spmv_smem_bytes;
@@ -186,6 +226,10 @@ struct acgb200_info {
                                                    codes into it (option "symdiag_codes"); 0: fp64 diagonals */
     int64_t spmv_symdiag_code_bytes;            /* the codes' bytes, one per element of the diagonals; 0: no codes */
     int mixed_reliable_updates;                 /* reliable updates of the last acgsolvercuda_solve_mixed */
+    /* the last acgsolvercuda_solve_chebyshev: its degree, the Jacobi-PCG steps of the interval estimate (0: none
+     * ran), 1 if a breakdown ended it, and the interval [cheb_lmin, cheb_lmax] used (0, 0: none) */
+    int cheb_degree, cheb_est_iterations, cheb_breakdown;
+    double cheb_lmin, cheb_lmax;
 };
 ACG_API int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info);
 
