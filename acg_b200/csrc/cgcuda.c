@@ -1531,7 +1531,7 @@ static int ensure_blocks(struct priv *pv, const struct acgsolvercuda *cg, int k,
 {
     if (!pv->d_ms) {
         CU(cudaMalloc((void **) &pv->d_ms, sizeof(*pv->d_ms)));
-        CU(cudaMemset(pv->d_ms, 0, sizeof(*pv->d_ms)));
+        CU(cudaMemsetAsync(pv->d_ms, 0, sizeof(*pv->d_ms), pv->stream));
         CU(cudaMallocHost((void **) &pv->h_ms, sizeof(*pv->h_ms)));
     }
     OK(build_ranges(pv, cg, errcode));
@@ -1546,7 +1546,7 @@ static int ensure_blocks(struct priv *pv, const struct acgsolvercuda *cg, int k,
     const size_t bytes = ((size_t) pv->nowned + 1) * (size_t) k * sizeof(double);
     for (int i = 0; i < 5; i++) {
         CU(cudaMalloc((void **) blk[i], bytes));
-        CU(cudaMemset(*blk[i], 0, bytes));
+        CU(cudaMemsetAsync(*blk[i], 0, bytes, pv->stream));
     }
     pv->mk = k;
     return ACG_SUCCESS;
@@ -2047,7 +2047,7 @@ static int mixed_alloc(struct priv *pv, const struct acgsolvercuda *cg, int *err
         /* four vectors of nowned + 2 floats, each starting on an 8-byte boundary (the kernels read pairs) */
         const size_t bytes = 4 * (((size_t) pv->nowned + 2) & ~(size_t) 1) * sizeof(float);
         CU(cudaMalloc((void **) &pv->d_f32, bytes));
-        CU(cudaMemset(pv->d_f32, 0, bytes));
+        CU(cudaMemsetAsync(pv->d_f32, 0, bytes, pv->stream));
     }
     if (!pv->have_franges) {
         int lanes = 0;
@@ -2260,7 +2260,7 @@ static int cheb_alloc(struct solvectx *c)
     if (!pv->d_cvec) {
         const size_t bytes = 5 * ((size_t) pv->nowned + 2) * sizeof(double);
         CU(cudaMalloc((void **) &pv->d_cvec, bytes));
-        CU(cudaMemset(pv->d_cvec, 0, bytes));
+        CU(cudaMemsetAsync(pv->d_cvec, 0, bytes, pv->stream));
     }
     if (pv->cheb_baddiag < 0) {
         struct acgb200_cstate cs;
