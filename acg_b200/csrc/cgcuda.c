@@ -186,7 +186,7 @@ struct priv {
     double last_blas_ms;                /* profiled fused-update time of the last solve */
     int last_spmv_n;
     int last_fused;                     /* the last solve ran the fused pipelined-CG iteration */
-    double *d_w2;                       /* fused pipelined CG: the second buffer of w (made at the first such solve) */
+    double *d_w2, *d_r2;                /* fused pipelined CG: the second buffers of w and r (made at the first such solve) */
     int commsize;                       /* ranks of the communicator given to acgsolvercuda_init */
     /* several right-hand sides (acgsolvercuda_solve_multi), made at the first multi-vector call */
     struct acgb200_mstate *d_ms, *h_ms; /* per-column scalars on the device / pinned staging */
@@ -316,7 +316,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
         if (pv->commstream) cudaStreamDestroy(pv->commstream);
         if (pv->redstream) cudaStreamDestroy(pv->redstream);
         if (pv->ev_red) cudaEventDestroy(pv->ev_red);
-        cudaFree(pv->d_b); cudaFree(pv->d_x); cudaFree(pv->d_w2);
+        cudaFree(pv->d_b); cudaFree(pv->d_x); cudaFree(pv->d_w2); cudaFree(pv->d_r2);
         cudaFree(pv->d_ms); cudaFreeHost(pv->h_ms); cudaFree(pv->d_ranges);
         cudaFree(pv->d_ss); cudaFreeHost(pv->h_ss);
         cudaFree(pv->d_ns); cudaFreeHost(pv->h_ns); cudaFree(pv->d_nw[0]); cudaFree(pv->d_nw[1]);
@@ -2615,12 +2615,14 @@ static int pipelined_iteration(struct solvectx *c, int k)
     const int s = k & 1, n = pv->nowned;
     const int peer = c->multi && c->p2p;
     if (c->fused) {
-        /* one GPU: iteration k gathers w from buffer k&1 and writes w_{k+1} into the other (DESIGN.md section 4a) */
+        /* one GPU: iteration k reads w and r from buffer k&1 and writes w_{k+1}, r_{k+1} into the other
+         * (DESIGN.md section 4a) */
         struct acgb200_pcgargs a;
         memset(&a, 0, sizeof(a));
         a.plan = &pv->plan; a.rowptr = cg->d_rowptr; a.colidx = cg->d_colidx; a.a = cg->d_a;
         a.w = s ? pv->d_w2 : cg->d_w; a.w_next = s ? cg->d_w : pv->d_w2;
-        a.q = cg->d_q; a.z = cg->d_z; a.t = cg->d_t; a.p = cg->d_p; a.r = cg->d_r; a.x = c->d_x;
+        a.r = s ? pv->d_r2 : cg->d_r; a.r_next = s ? cg->d_r : pv->d_r2;
+        a.q = cg->d_q; a.z = cg->d_z; a.t = cg->d_t; a.p = cg->d_p; a.x = c->d_x;
         a.st = st; a.cin = s; a.vec_evict_first = cfg.pcg_evict_first;
         /* the whole iteration is timed as the product: no separate update time on this path */
         prof_mark(c, &pv->gemv);
@@ -2694,12 +2696,18 @@ int acgsolvercuda_solve_pipelined(
         CU(cudaMalloc((void **) &pv->d_w2, ((size_t) pv->nvec + 2) * sizeof(double)));
         CU(cudaMemsetAsync(pv->d_w2, 0, ((size_t) pv->nvec + 2) * sizeof(double), pv->stream));
     }
+    if (c.fused && !pv->d_r2) {
+        CU(cudaMalloc((void **) &pv->d_r2, ((size_t) pv->nvec + 2) * sizeof(double)));
+        CU(cudaMemsetAsync(pv->d_r2, 0, ((size_t) pv->nvec + 2) * sizeof(double), pv->stream));
+    }
     if (c.p2p) OK(acgcomm_barrier(pv->stream, comm, errcode));     /* as in acgsolvercuda_solvempi */
     if (warmup > 0) {
         memset(&h, 0, sizeof(h));
         h.maxits = warmup;
         for (int s = 0; s < 2; s++) { h.gd_loc[s][0] = h.gd[s][0] = 1; h.gd_loc[s][1] = h.gd[s][1] = 1; h.prev[s][0] = h.prev[s][1] = INFINITY; }
         OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        /* x on r: the fused loop also writes d_r2, and the set-up below rewrites both r buffers before the
+         * solve reads them (d_r from b - A x0, d_r2 in iteration 0) */
         double *xsave = c.d_x; c.d_x = cg->d_r;
         if (c.p2p) {
             OK(acgb200_p2p_begin(&pv->p2p, warmup, pv->stream));
@@ -2751,6 +2759,12 @@ int acgsolvercuda_solve_pipelined(
             OK(post(&c, 0, 0, cg->d_w, -1, NULL, 0, 0, 0, 0));
         }
         OK(iterate(&c, maxits, tol > 0, pipelined_iteration));
+        if (c.fused) {
+            /* an even last update left p, x behind and r_{k+1} in d_r2; launched whatever the parity, so the
+             * launch count of a solve does not depend on where it stopped */
+            KL(acgb200_pcg_fused_finish(n, st, c.issued & 1, cg->d_r, pv->d_r2, cg->d_p, c.d_x, pv->stream));
+            c.launches += 1;
+        }
         OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
         const struct acgb200_ctrl cw = h.ctrl[c.fused ? c.issued & 1 : 0];
         cg->niterations = cw.iter;

@@ -233,23 +233,36 @@ __device__ __forceinline__ PcgStep pcg_step(const acgb200_devstate *st, int iter
     return o;
 }
 
-/* z=q+beta z; t=w+beta t; p=r+beta p; x+=alpha p; r-=alpha t; w'=w-alpha z for row i (the fma chain of
- * pcg_update_kernel), w' into the other buffer; gamma'=(r,r), delta'=(w',r) accumulate in g2, d2 */
-__device__ __forceinline__ void pcg_row(int i, double qi, double wi, const PcgStep &k, double *__restrict__ z,
-                                        double *__restrict__ t, double *__restrict__ p, double *__restrict__ r,
+/*
+ * Row i of update k, the fma chain of pcg_update_kernel: z=q+beta z; t=w+beta t; p=r+beta p; x+=alpha p;
+ * r-=alpha t; w'=w-alpha z, w' into the other buffer; gamma'=(r,r), delta'=(w',r) accumulate in g2, d2.
+ * p and x feed nothing but themselves, so they lag (DESIGN section 4a): an even k reads r_k from r, writes
+ * r_{k+1} into r_next and leaves p and x alone; an odd k reads r_k from r and r_{k-1} from r_next, forms
+ * p_{k-1} and p_k and both x updates -- the same FMAs in the same order -- and writes r_{k+1} over r_{k-1}.
+ * lag (odd k only): {alpha_{k-1}, beta_{k-1}} in memory that the kernel does not write; st_vec clobbers
+ * memory, so they are read per row rather than held in registers through the product loop.
+ */
+template <bool ODD>
+__device__ __forceinline__ void pcg_row(int i, double qi, double wi, double alpha, double beta, const double *lag,
+                                        double *__restrict__ z, double *__restrict__ t, double *__restrict__ p,
+                                        const double *__restrict__ r, double *__restrict__ r_next,
                                         double *__restrict__ x, double *__restrict__ w_next, uint64_t pol,
                                         double &g2, double &d2)
 {
-    const double zi = ld_vec(z + i, pol), ti = ld_vec(t + i, pol), pi = ld_vec(p + i, pol);
-    const double ri = ld_vec(r + i, pol), xi = ld_vec(x + i, pol);
-    const double zv = fma(k.beta, zi, qi);
-    const double tv = fma(k.beta, ti, wi);
-    const double pv = fma(k.beta, pi, ri);
-    const double rv = fma(-k.alpha, tv, ri);
-    const double wv = fma(-k.alpha, zv, wi);
-    st_vec(z + i, zv, pol); st_vec(t + i, tv, pol); st_vec(p + i, pv, pol);
-    st_vec(x + i, fma(k.alpha, pv, xi), pol);
-    st_vec(r + i, rv, pol);
+    const double zi = ld_vec(z + i, pol), ti = ld_vec(t + i, pol), ri = ld_vec(r + i, pol);
+    const double zv = fma(beta, zi, qi);
+    const double tv = fma(beta, ti, wi);
+    const double rv = fma(-alpha, tv, ri);
+    const double wv = fma(-alpha, zv, wi);
+    if (ODD) {
+        const double pi = ld_vec(p + i, pol), rp = ld_vec(r_next + i, pol), xi = ld_vec(x + i, pol);
+        const double pl = fma(lag[1], pi, rp);
+        const double pv = fma(beta, pl, ri);
+        st_vec(p + i, pv, pol);
+        st_vec(x + i, fma(alpha, pv, fma(lag[0], pl, xi)), pol);
+    }
+    st_vec(z + i, zv, pol); st_vec(t + i, tv, pol);
+    st_vec(r_next + i, rv, pol);
     st_vec(w_next + i, wv, pol);
     g2 = fma(rv, rv, g2);
     d2 = fma(wv, rv, d2);
@@ -802,8 +815,9 @@ struct SymdiagParams {
     acgb200_ctrl *ctrl_out;
     acgb200_devstate *st;
     int housekeeping;
-    /* pipelined-CG epilogue (PCG): x above is w_k; z, t, p, r, xs updated in place, w_{k+1} into w_next */
-    double *z, *t, *p, *r, *xs, *w_next;
+    /* pipelined-CG epilogue (PCG): x above is w_k; z, t, p, xs updated in place, w_{k+1} into w_next, r_k
+     * read from r and r_{k+1} written to r_next (pcg_row) */
+    double *z, *t, *p, *r, *r_next, *xs, *w_next;
     int vec_evict_first;
 };
 
@@ -824,6 +838,7 @@ struct SymdiagParams {
  * and goes straight into the update (pcg_row) instead of to memory; the kernel is the iteration's last, so
  * block 0 advances the control word and zeroes ring slot (k+2) % 3 while every CTA adds into (k+1) % 3.
  * A met convergence test returns before the product.  At most 40 registers: 12 CTAs of 128 threads.
+ * ODD: the parity of k, which decides whether the row also catches up on p and x (pcg_row).
  *
  * V: double reads the fp64 diagonals (hval); uint8_t reads one code per element (hcode) and decodes it from
  * a copy of the value table in shared memory just before the FMAs -- the same double, bit for bit, so the
@@ -878,13 +893,14 @@ __device__ __forceinline__ double symdiag_row_sum(const SymdiagParams &P, const 
     return sum;
 }
 
-template <int UB, int T, bool PCG, typename V, typename X = double>
+template <int UB, int T, bool PCG, typename V, typename X = double, bool ODD = false>
 __global__ void __launch_bounds__(T, PCG ? 1536 / T : 0)
 spmv_symdiag_kernel(const SymdiagParams P)
 {
     constexpr bool CODED = std::is_same<V, uint8_t>::value;
     constexpr bool F32 = std::is_same<X, float>::value;
     static_assert(!(F32 && PCG), "the fused pipelined-CG epilogue is fp64 only");
+    static_assert(PCG || !ODD, "parity only selects the fused epilogue's form");
     __shared__ int2 tab_s[ACGB200_SYMDIAG_MAX];
     __shared__ double vtab_s[CODED ? 256 : 1];
     __shared__ double red[T / 32];
@@ -900,7 +916,10 @@ spmv_symdiag_kernel(const SymdiagParams P)
                 const int s = gate.iter & 1, z = (gate.iter + 2) % 3;
                 P.st->gd_loc[z][0] = 0.0; P.st->gd_loc[z][1] = 0.0;
                 if (k.conv) { c.done = 1; P.st->final_rr = k.gamma; }
-                else { c.iter = gate.iter + 1; P.st->prev[s ^ 1][0] = k.gamma; P.st->prev[s ^ 1][1] = k.alpha; }
+                else {
+                    c.iter = gate.iter + 1;
+                    P.st->prev[s ^ 1][0] = k.gamma; P.st->prev[s ^ 1][1] = k.alpha; P.st->prev[s ^ 1][2] = k.beta;
+                }
             }
             *P.ctrl_out = c;
         }
@@ -914,6 +933,10 @@ spmv_symdiag_kernel(const SymdiagParams P)
         }
     }
     if (!gate.active) return;
+    /* ODD: {alpha_k, beta_k, alpha_{k-1}, beta_{k-1}} for pcg_row, from shared memory rather than registers
+     * (the second pair would make the fp64 loops spill); prev[1] is written by even iterations only */
+    __shared__ double ks_s[ODD ? 4 : 1];
+    if (ODD && tid == 0) { ks_s[0] = k.alpha; ks_s[1] = k.beta; ks_s[2] = P.st->prev[1][1]; ks_s[3] = P.st->prev[1][2]; }
     if (tid < P.no) tab_s[tid] = make_int2(P.tab[tid].voff, P.tab[tid].coff);
     if (CODED) for (int i = tid; i < P.ncodes; i += T) vtab_s[i] = __ldg(P.vtab + i);
     __syncthreads();
@@ -933,7 +956,8 @@ spmv_symdiag_kernel(const SymdiagParams P)
         const double sum = symdiag_row_sum<UB, V, X>(P, tab_s, vtab_s, row, pol, cmax, L);
         if (PCG) {
             /* w_i was gathered by this row a moment ago: an L1 hit, not a third stream */
-            pcg_row(row, sum, __ldg(P.x + row), k, P.z, P.t, P.p, P.r, P.xs, P.w_next, vpol, dot, dot2);
+            pcg_row<ODD>(row, sum, __ldg(P.x + row), ODD ? ks_s[0] : k.alpha, ODD ? ks_s[1] : k.beta, ks_s + 2,
+                         P.z, P.t, P.p, P.r, P.r_next, P.xs, P.w_next, vpol, dot, dot2);
         } else if (F32) {
             const X ys = (X) sum;
             sd_vec<X>(P.y)[row] = ys;
@@ -1716,11 +1740,13 @@ pcg_update_kernel(int n, acgb200_devstate *st, int cin, int cout, int multi, acg
  * row ranges of the tile plan, one CTA per tile and trip.  Adds into the same ring slot as the fused kernel,
  * which runs after it and advances the control word; this one only forwards it. */
 #define PCG_TAIL_THREADS 128
+template <bool ODD>
 __global__ void __launch_bounds__(PCG_TAIL_THREADS)
 pcg_tail_update_kernel(const acgb200_tile *__restrict__ tiles, int ntiles, acgb200_devstate *st,
                        const acgb200_ctrl *cin, acgb200_ctrl *cout, const double *__restrict__ q,
                        const double *__restrict__ w, double *__restrict__ w_next, double *__restrict__ z,
-                       double *__restrict__ t, double *__restrict__ p, double *__restrict__ r, double *__restrict__ x)
+                       double *__restrict__ t, double *__restrict__ p, const double *__restrict__ r,
+                       double *__restrict__ r_next, double *__restrict__ x)
 {
     __shared__ double red[PCG_TAIL_THREADS / 32];
     pdl_prologue();
@@ -1734,7 +1760,7 @@ pcg_tail_update_kernel(const acgb200_tile *__restrict__ tiles, int ntiles, acgb2
     for (int b = blockIdx.x; b < ntiles; b += gridDim.x) {
         const acgb200_tile tl = tiles[b];
         for (int i = tl.row_begin + (int) threadIdx.x; i < tl.row_begin + tl.nrows; i += PCG_TAIL_THREADS)
-            pcg_row(i, q[i], w[i], k, z, t, p, r, x, w_next, pol, g2, d2);
+            pcg_row<ODD>(i, q[i], w[i], k.alpha, k.beta, &st->prev[1][1], z, t, p, r, r_next, x, w_next, pol, g2, d2);
     }
     g2 = block_sum(g2, red);
     d2 = block_sum(d2, red);
@@ -1742,6 +1768,24 @@ pcg_tail_update_kernel(const acgb200_tile *__restrict__ tiles, int ntiles, acgb2
         double *acc = st->gd_loc[(g.iter + 1) % 3];
         atomicAdd(&acc[0], g2);
         atomicAdd(&acc[1], d2);
+    }
+}
+
+/* Fused pipelined CG, after the loop: the final control word counts the updates m.  If m is odd, the last
+ * one (m - 1, even) left its p and x updates to an iteration that did not run, and its r_m sits in r2: form
+ * p_{m-1} = r_{m-1} + beta_{m-1} p and x += alpha_{m-1} p_{m-1} (pcg_row's FMAs), and move r_m into r. */
+__global__ void __launch_bounds__(BLAS1_THREADS)
+pcg_fused_finish_kernel(int n, const acgb200_devstate *st, int cfin, double *__restrict__ r,
+                        const double *__restrict__ r2, double *__restrict__ p, double *__restrict__ x)
+{
+    const int m = st->ctrl[cfin].iter;
+    if (!(m & 1)) return;
+    const double alpha = st->prev[1][1], beta = st->prev[1][2];
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const double pv = fma(beta, p[i], r[i]);
+        p[i] = pv;
+        x[i] = fma(alpha, pv, x[i]);
+        r[i] = r2[i];
     }
 }
 
@@ -2937,20 +2981,22 @@ static slice_fn slice_variant(int UB, int T, int EXC)
 typedef void (*symdiag_fn)(const SymdiagParams);
 
 /* the mirrored-diagonal kernel for exactly the (UB, T) pairs of slice_variant; pcg: with the fused
- * pipelined-CG epilogue; coded: reading one-byte codes (the plan's symdiag_codes > 0) */
-static symdiag_fn symdiag_variant(int UB, int T, bool pcg, bool coded)
+ * pipelined-CG epilogue, odd: its form for odd iterations; coded: reading one-byte codes (the plan's
+ * symdiag_codes > 0) */
+static symdiag_fn symdiag_variant(int UB, int T, bool pcg, bool odd, bool coded)
 {
-#define X(u, t) if (UB == u && T == t) \
-        return coded ? (pcg ? spmv_symdiag_kernel<u, t, true, uint8_t> : spmv_symdiag_kernel<u, t, false, uint8_t>) \
-                     : (pcg ? spmv_symdiag_kernel<u, t, true, double> : spmv_symdiag_kernel<u, t, false, double>);
+#define V(u, t, c) (pcg ? (odd ? spmv_symdiag_kernel<u, t, true, c, double, true> : spmv_symdiag_kernel<u, t, true, c>) \
+                        : spmv_symdiag_kernel<u, t, false, c>)
+#define X(u, t) if (UB == u && T == t) return coded ? V(u, t, uint8_t) : V(u, t, double);
     X(5, 128) X(7, 128) X(8, 128) X(9, 128) X(7, 256) X(8, 256) X(9, 256)
 #undef X
+#undef V
     return NULL;
 }
 
-static symdiag_fn symdiag_variant(const acgb200_spmvplan *pl, bool pcg)
+static symdiag_fn symdiag_variant(const acgb200_spmvplan *pl, bool pcg, bool odd = false)
 {
-    return symdiag_variant(pl->slice_ub, pl->slice_threads, pcg, pl->symdiag_codes > 0);
+    return symdiag_variant(pl->slice_ub, pl->slice_threads, pcg, odd, pl->symdiag_codes > 0);
 }
 
 /* the float-vector product of the mixed-precision solve, for the same (UB, T) pairs */
@@ -3073,11 +3119,15 @@ extern "C" int acgb200_spmv_configure(acgb200_spmvplan *pl)
         pl->slice_grid = (int) (sgrid < 1 ? 1 : sgrid);
         pl->pcg_grid = 0;
         if (pl->symdiag_nd > 0) {
-            /* the fused pipelined-CG kernel: the same grid, unless its registers allow fewer CTAs */
-            int fper = 0;
-            err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fper, (const void *) symdiag_variant(pl, true),
+            /* the fused pipelined-CG kernel: the same grid, unless the registers of either parity's form
+             * allow fewer CTAs */
+            int fper = 0, oper = 0;
+            err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fper, (const void *) symdiag_variant(pl, true, false),
                                                                 pl->slice_threads, 0);
+            if (!err) err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&oper, (const void *) symdiag_variant(pl, true, true),
+                                                                          pl->slice_threads, 0);
             if (err) return (int) err;
+            if (oper < fper) fper = oper;
             const long long fgrid = (long long) acgb200_num_sms() * (fper < 1 ? 1 : fper);
             pl->pcg_grid = (int) (fgrid < pl->slice_grid ? fgrid : pl->slice_grid);
         }
@@ -3281,10 +3331,11 @@ extern "C" int acgb200_pcg_fused_launch(const acgb200_pcgargs *a, cudaStream_t s
         long long grid = pl->ntiles;
         const long long cap = (long long) acgb200_num_sms() * 8;
         if (grid > cap) grid = cap;
-        const cudaError_t le = launch_chain(pcg_tail_update_kernel, (int) grid, PCG_TAIL_THREADS, 0, stream,
+        const cudaError_t le = launch_chain(a->cin ? pcg_tail_update_kernel<true> : pcg_tail_update_kernel<false>,
+                                            (int) grid, PCG_TAIL_THREADS, 0, stream,
                                             (const acgb200_tile *) pl->d_tiles, pl->ntiles, a->st,
                                             (const acgb200_ctrl *) &ctrl[2], &ctrl[3], (const double *) a->q, a->w,
-                                            a->w_next, a->z, a->t, a->p, a->r, a->x);
+                                            a->w_next, a->z, a->t, a->p, (const double *) a->r, a->r_next, a->x);
         if (le) return (int) le;
         fin = 3;
     }
@@ -3293,11 +3344,20 @@ extern "C" int acgb200_pcg_fused_launch(const acgb200_pcgargs *a, cudaStream_t s
     symdiag_params(pl, S);
     S.x = a->w; S.mode = SPMV_Y_AX;
     S.ctrl_in = &ctrl[fin]; S.ctrl_out = &ctrl[cout]; S.st = a->st;
-    S.z = a->z; S.t = a->t; S.p = a->p; S.r = a->r; S.xs = a->x; S.w_next = a->w_next;
+    S.z = a->z; S.t = a->t; S.p = a->p; S.r = a->r; S.r_next = a->r_next; S.xs = a->x; S.w_next = a->w_next;
     S.vec_evict_first = a->vec_evict_first;
-    const cudaError_t le = launch_chain(symdiag_variant(pl, true), pl->pcg_grid, pl->slice_threads,
+    const cudaError_t le = launch_chain(symdiag_variant(pl, true, a->cin != 0), pl->pcg_grid, pl->slice_threads,
                                         (size_t) 0, stream, S);
     if (le) return (int) le;
+    return (int) cudaGetLastError();
+}
+
+extern "C" int acgb200_pcg_fused_finish(int n, const acgb200_devstate *st, int cfin, double *r, const double *r2,
+                                        double *p, double *x, cudaStream_t stream)
+{
+    static int occ = 0;
+    pcg_fused_finish_kernel<<<blas1_grid(n, (const void *) pcg_fused_finish_kernel, &occ), BLAS1_THREADS, 0, stream>>>(
+        n, st, cfin, r, r2, p, x);
     return (int) cudaGetLastError();
 }
 

@@ -23,17 +23,20 @@ int64_t acgb200_spmv_min_bytes(const struct acgb200_spmvplan *pl)
            + pl->slice_excnnz * 4 + pl->slice_exc * 8;
 }
 
-/* fused pipelined CG, per covered row: the stored diagonals, w_i, reads of z t p r x, writes of z t p x r w' */
+/* fused pipelined CG with every update done in its own iteration, per covered row: the stored diagonals,
+ * w_i, reads of z t p r x, writes of z t p x r w' */
 int64_t acgb200_pcg_fused_min_bytes(const struct acgb200_spmvplan *pl)
 {
     return (int64_t) pl->slice_rows * (symdiag_elem_bytes(pl) * pl->symdiag_nd + 96);
 }
 
-/* the whole fused iteration: the tile kernel's product, the tile rows' update (7 reads, 6 writes), the fused launch */
+/* the whole fused iteration as it runs, p and x updated every second iteration: the tile kernel's product,
+ * then per row the mean of an even and an odd update.  Covered rows: w_i, z t r read, z t r w' written
+ * (64), and w_i, z t r r_prev p x read, z t p x r w' written (104).  Tile rows: q_i read on top (72, 112). */
 int64_t acgb200_pcg_iteration_min_bytes(const struct acgb200_spmvplan *pl)
 {
     const int64_t tnnz = pl->nnz - pl->slice_nnz, trows = pl->nrows - pl->slice_rows;
-    return tnnz * 12 + trows * (20 + 104) + acgb200_pcg_fused_min_bytes(pl);
+    return tnnz * 12 + trows * (20 + 92) + (int64_t) pl->slice_rows * (symdiag_elem_bytes(pl) * pl->symdiag_nd + 84);
 }
 
 /*
