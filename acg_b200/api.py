@@ -133,7 +133,8 @@ class acgb200_info(C.Structure):
         [("spmv_symdiag_codes", C.c_int), ("spmv_symdiag_code_bytes", C.c_int64)] + \
         [("mixed_reliable_updates", C.c_int)] + \
         [("cheb_degree", C.c_int), ("cheb_est_iterations", C.c_int), ("cheb_breakdown", C.c_int),
-         ("cheb_lmin", C.c_double), ("cheb_lmax", C.c_double)]
+         ("cheb_lmin", C.c_double), ("cheb_lmax", C.c_double)] + \
+        [("pcg_group", C.c_int)]
 
 
 class acgb200_colstats(C.Structure):

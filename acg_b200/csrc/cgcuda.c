@@ -42,6 +42,7 @@
 /* ------------------------------------------------------------------------ */
 
 #define SPMV_MAX_STAGES_HOST 8      /* SPMV_MAX_STAGES of kernels.cu */
+#define PCG_GROUP_DEFAULT 16        /* option pcg_group: see the measurements in DESIGN.md section 4a */
 
 static struct {
     int profile;        /* record CUDA events around each kernel class */
@@ -67,9 +68,13 @@ static struct {
     int pcg_fused;      /* 1: pipelined CG runs each iteration's product and update in one kernel where the plan allows
                          * (one GPU, mirrored diagonals; DESIGN.md section 4a), 0: off (A/B) */
     int pcg_evict_first;   /* 1: L2 evict-first policy on the fused kernel's vector streams (A/B) */
+    int pcg_group;      /* the fused iteration's p and x updates are done once per this many iterations: 2, 4, 8 or 16
+                         * (DESIGN.md section 4a) */
     int loaded;
 } cfg = { .check_every = 8, .graph = 1, .redstream = 1, .p2p = 1, .p2p_fuse = 1, .spmv_slices = 1, .spmv_merge = -1,
-          .spmv_symdiag = 1, .symdiag_codes = 1, .pcg_fused = 1, .pcg_evict_first = 1 };
+          .spmv_symdiag = 1, .symdiag_codes = 1, .pcg_fused = 1, .pcg_evict_first = 1, .pcg_group = PCG_GROUP_DEFAULT };
+
+static int pcg_group_valid(int m) { return m == 2 || m == 4 || m == 8 || m == ACGB200_PCG_GROUP_MAX; }
 
 static void cfg_load(void)
 {
@@ -107,6 +112,7 @@ static void cfg_load(void)
     if ((s = getenv("ACGB200_SYMDIAG_CODES"))) cfg.symdiag_codes = atoi(s);
     if ((s = getenv("ACGB200_PCG_FUSED"))) cfg.pcg_fused = atoi(s);
     if ((s = getenv("ACGB200_PCG_EVICT_FIRST"))) cfg.pcg_evict_first = atoi(s);
+    if ((s = getenv("ACGB200_PCG_GROUP")) && pcg_group_valid(atoi(s))) cfg.pcg_group = atoi(s);
     acgb200_blas1_set_ctas_per_sm(cfg.blas1_ctas);
     acgb200_set_pdl(cfg.pdl);
 }
@@ -144,6 +150,7 @@ int acgb200_set_option(const char *key, int value)
     else if (!strcmp(key, "symdiag_codes")) cfg.symdiag_codes = value;
     else if (!strcmp(key, "pcg_fused")) cfg.pcg_fused = value;
     else if (!strcmp(key, "pcg_evict_first")) cfg.pcg_evict_first = value;
+    else if (!strcmp(key, "pcg_group") && pcg_group_valid(value)) cfg.pcg_group = value;
     else return ACG_ERR_INVALID_VALUE;
     return ACG_SUCCESS;
 }
@@ -174,7 +181,7 @@ struct priv {
     struct acgcomm redcomm;             /* private duplicate of the caller's communicator for reductions */
     int have_redcomm;
     double *d_b, *d_x;                  /* right-hand side / solution on the device, kept between solves */
-    cudaGraphExec_t graph[NKINDS];      /* per solve kind: two iterations (parity 0 then 1) */
+    cudaGraphExec_t graph[NKINDS];      /* per solve kind: two iterations (parity 0 then 1), or a fused group */
     int graph_sig[NKINDS];              /* loop configuration each cached graph was captured with (graph_signature) */
     int graph_launches[NKINDS];         /* kernel/NCCL launches inside one replay */
     double last_h2d_ms, last_d2h_ms;    /* host time spent before / after the solve window */
@@ -186,7 +193,12 @@ struct priv {
     double last_blas_ms;                /* profiled fused-update time of the last solve */
     int last_spmv_n;
     int last_fused;                     /* the last solve ran the fused pipelined-CG iteration */
-    double *d_w2, *d_r2;                /* fused pipelined CG: the second buffers of w and r (made at the first such solve) */
+    /* fused pipelined CG: the second buffer of w, and slots 1 ... r_slots of the r ring, r_stride doubles apart
+     * (made at the first such solve, the ring grown with the group) */
+    double *d_w2, *d_rring;
+    size_t r_stride;
+    int r_slots;
+    int last_group;                     /* the group of the last fused solve */
     int commsize;                       /* ranks of the communicator given to acgsolvercuda_init */
     /* several right-hand sides (acgsolvercuda_solve_multi), made at the first multi-vector call */
     struct acgb200_mstate *d_ms, *h_ms; /* per-column scalars on the device / pinned staging */
@@ -316,7 +328,7 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
         if (pv->commstream) cudaStreamDestroy(pv->commstream);
         if (pv->redstream) cudaStreamDestroy(pv->redstream);
         if (pv->ev_red) cudaEventDestroy(pv->ev_red);
-        cudaFree(pv->d_b); cudaFree(pv->d_x); cudaFree(pv->d_w2); cudaFree(pv->d_r2);
+        cudaFree(pv->d_b); cudaFree(pv->d_x); cudaFree(pv->d_w2); cudaFree(pv->d_rring);
         cudaFree(pv->d_ms); cudaFreeHost(pv->h_ms); cudaFree(pv->d_ranges);
         cudaFree(pv->d_ss); cudaFreeHost(pv->h_ss);
         cudaFree(pv->d_ns); cudaFreeHost(pv->h_ns); cudaFree(pv->d_nw[0]); cudaFree(pv->d_nw[1]);
@@ -911,6 +923,7 @@ struct solvectx {
     enum solve_kind kind;     /* the loop iterate() runs, and so its graph slot */
     int fused;                /* pipelined loop: one fused iteration (acgb200_pcg_fused_launch); its control word
                                * alternates between ctrl[0] and ctrl[1] by iteration parity */
+    int group;                /* fused pipelined loop: its group of iterations, even (DESIGN.md section 4a) */
     int issued;               /* iterations iterate() issued, inactive ones included */
     double t0;                /* host clock at the start of the solve window */
     /* Chebyshev loop: the degree, the fused inner step (acgb200_cheb_fused_step), the start's and the steps'
@@ -965,6 +978,7 @@ static int window_open(struct solvectx *c, int maxits, double atol, double rtol,
     cg->residualatol = atol; cg->residualrtol = rtol;
     /* what acgsolvercuda_info reports of the last solve, whichever entry point runs it */
     pv->last_fused = c->fused;
+    if (c->fused) pv->last_group = c->group;
     pv->last_mixed_updates = 0;
     pv->last_cheb_degree = pv->last_cheb_est = pv->last_cheb_breakdown = 0;
     pv->last_cheb_lmin = pv->last_cheb_lmax = 0;
@@ -1232,10 +1246,11 @@ static double threshold(double atol, double rtol, double r0nrm2)
     return t;
 }
 
-/* Capture iterations (parity 0, parity 1) of `issue` into a graph.  All
+/* Capture iterations g ... 2g - 1 of `issue` into a graph (g = graph_group).  All
  * pointers the kernels and NCCL calls use are fixed for the life of the solver
- * and the iteration index only enters through its parity, so one two-iteration
- * graph serves the whole solve (and later solves). */
+ * and the iteration index only enters through its parity, or on the fused
+ * pipelined path through its place in the group, so one graph of a group of
+ * iterations serves the whole solve (and later solves). */
 /* everything besides the (fixed) pointers and the solve kind (its own slot) that decides which kernels and
  * NCCL calls an iteration issues: a cached graph is only replayed for the configuration it was captured with
  * (options can change between two solves on one solver) */
@@ -1243,10 +1258,13 @@ static int graph_signature(const struct solvectx *c)
 {
     return 1 | (c->multi ? 2 : 0) | (c->p2p ? 4 : 0) | (c->pv->p2p.h_desc.fuse ? 8 : 0) | (cfg.pdl ? 16 : 0)
            | (cfg.redstream ? 32 : 0) | (c->pv->have_redcomm ? 64 : 0) | (c->mk << 8) | (c->fused ? 1 << 16 : 0)
-           | (c->cheb_degree << 18) | (c->cheb_fused ? 1 << 23 : 0);
+           | (c->cheb_degree << 18) | (c->cheb_fused ? 1 << 23 : 0) | (c->fused ? c->group << 24 : 0);
 }
 
-static int capture_pair(struct solvectx *c, int (*issue)(struct solvectx *, int))
+/* iterations per graph replay: the fused pipelined loop's group, two for every other loop */
+static int graph_group(const struct solvectx *c) { return c->fused ? c->group : 2; }
+
+static int capture_group(struct solvectx *c, int (*issue)(struct solvectx *, int))
 {
     struct priv *pv = c->pv;
     int *errcode = c->errcode;
@@ -1257,8 +1275,8 @@ static int capture_pair(struct solvectx *c, int (*issue)(struct solvectx *, int)
     cudaGraph_t g = NULL;
     c->capturing = 1;
     CU(cudaStreamBeginCapture(pv->stream, cudaStreamCaptureModeThreadLocal));
-    int err = issue(c, 2);
-    if (!err) err = issue(c, 3);
+    int err = 0;
+    for (int k = graph_group(c); k < 2 * graph_group(c) && !err; k++) err = issue(c, k);
     cudaError_t e = cudaStreamEndCapture(pv->stream, &g);
     c->capturing = 0;
     pv->graph_launches[kind] = c->launches - before;
@@ -1273,13 +1291,17 @@ static int capture_pair(struct solvectx *c, int (*issue)(struct solvectx *, int)
 }
 
 /* Run `issue(c,k)` for k < maxits, polling the device control word.  The
- * first two iterations are issued directly (they also serve as the un-captured
- * first use of every NCCL path), the rest as replays of the two-iteration graph. */
+ * first group of iterations (two, or the fused pipelined loop's group) is
+ * issued directly (it also serves as the un-captured first use of every NCCL
+ * path), then whole groups as replays of the graph, and the rest directly.
+ * A replay may run past check_every: a converged solve then issues up to a
+ * group of iterations that return at once. */
 static int iterate(struct solvectx *c, int maxits, int poll, int (*issue)(struct solvectx *, int))
 {
     struct priv *pv = c->pv;
     int *errcode = c->errcode;
     const enum solve_kind kind = c->kind;
+    const int group = graph_group(c);
     int issued = 0, slot = 0, have_prev = 0, since_poll = 0;
     /* Replays are used on one GPU and with the peer-memory exchange (kernel nodes
      * only).  With the NCCL exchange the iteration also contains collectives on
@@ -1288,11 +1310,11 @@ static int iterate(struct solvectx *c, int maxits, int poll, int (*issue)(struct
      * on request (option "graph" = 2). */
     const int use_graph = cfg.graph && !cfg.profile && maxits >= 6 && (!c->multi || c->p2p || cfg.graph >= 2);
     while (issued < maxits) {
-        if (use_graph && issued >= 2 && maxits - issued >= 2) {
-            if (!pv->graph[kind] || pv->graph_sig[kind] != graph_signature(c)) OK(capture_pair(c, issue));
+        if (use_graph && issued >= group && issued % group == 0 && maxits - issued >= group) {
+            if (!pv->graph[kind] || pv->graph_sig[kind] != graph_signature(c)) OK(capture_group(c, issue));
             CU(cudaGraphLaunch(pv->graph[kind], pv->stream));
             c->launches += pv->graph_launches[kind];
-            issued += 2; since_poll += 2;
+            issued += group; since_poll += group;
         } else {
             OK(issue(c, issued));
             issued += 1; since_poll += 1;
@@ -2615,13 +2637,17 @@ static int pipelined_iteration(struct solvectx *c, int k)
     const int s = k & 1, n = pv->nowned;
     const int peer = c->multi && c->p2p;
     if (c->fused) {
-        /* one GPU: iteration k reads w and r from buffer k&1 and writes w_{k+1}, r_{k+1} into the other
-         * (DESIGN.md section 4a) */
+        /* one GPU: iteration k gathers w from buffer k&1 and writes w_{k+1} into the other; it reads r_k from
+         * ring slot k % m and writes r_{k+1} into slot (k+1) % m, and the last of each group of m also
+         * updates p and x for the whole group (DESIGN.md section 4a) */
+        const int m = c->group, j = k % m, jn = (j + 1) % m;
         struct acgb200_pcgargs a;
         memset(&a, 0, sizeof(a));
         a.plan = &pv->plan; a.rowptr = cg->d_rowptr; a.colidx = cg->d_colidx; a.a = cg->d_a;
         a.w = s ? pv->d_w2 : cg->d_w; a.w_next = s ? cg->d_w : pv->d_w2;
-        a.r = s ? pv->d_r2 : cg->d_r; a.r_next = s ? cg->d_r : pv->d_r2;
+        a.r = j ? pv->d_rring + (size_t) (j - 1) * pv->r_stride : cg->d_r;
+        a.r_next = jn ? pv->d_rring + (size_t) (jn - 1) * pv->r_stride : cg->d_r;
+        a.r_ring = pv->d_rring; a.r_stride = pv->r_stride; a.group = m; a.catchup = j == m - 1;
         a.q = cg->d_q; a.z = cg->d_z; a.t = cg->d_t; a.p = cg->d_p; a.x = c->d_x;
         a.st = st; a.cin = s; a.vec_evict_first = cfg.pcg_evict_first;
         /* the whole iteration is timed as the product: no separate update time on this path */
@@ -2696,9 +2722,16 @@ int acgsolvercuda_solve_pipelined(
         CU(cudaMalloc((void **) &pv->d_w2, ((size_t) pv->nvec + 2) * sizeof(double)));
         CU(cudaMemsetAsync(pv->d_w2, 0, ((size_t) pv->nvec + 2) * sizeof(double), pv->stream));
     }
-    if (c.fused && !pv->d_r2) {
-        CU(cudaMalloc((void **) &pv->d_r2, ((size_t) pv->nvec + 2) * sizeof(double)));
-        CU(cudaMemsetAsync(pv->d_r2, 0, ((size_t) pv->nvec + 2) * sizeof(double), pv->stream));
+    if (c.fused) c.group = cfg.pcg_group;
+    if (c.fused && pv->r_slots < c.group - 1) {
+        /* slots 1 ... m-1 of the r ring (slot 0 is d_r), each on a 256-byte boundary */
+        const size_t stride = ((size_t) pv->nvec + 2 + 31) & ~(size_t) 31;
+        CU(cudaStreamSynchronize(pv->stream));
+        cudaFree(pv->d_rring);
+        pv->d_rring = NULL; pv->r_slots = 0;
+        CU(cudaMalloc((void **) &pv->d_rring, (size_t) (c.group - 1) * stride * sizeof(double)));
+        CU(cudaMemsetAsync(pv->d_rring, 0, (size_t) (c.group - 1) * stride * sizeof(double), pv->stream));
+        pv->r_stride = stride; pv->r_slots = c.group - 1;
     }
     if (c.p2p) OK(acgcomm_barrier(pv->stream, comm, errcode));     /* as in acgsolvercuda_solvempi */
     if (warmup > 0) {
@@ -2706,8 +2739,8 @@ int acgsolvercuda_solve_pipelined(
         h.maxits = warmup;
         for (int s = 0; s < 2; s++) { h.gd_loc[s][0] = h.gd[s][0] = 1; h.gd_loc[s][1] = h.gd[s][1] = 1; h.prev[s][0] = h.prev[s][1] = INFINITY; }
         OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
-        /* x on r: the fused loop also writes d_r2, and the set-up below rewrites both r buffers before the
-         * solve reads them (d_r from b - A x0, d_r2 in iteration 0) */
+        /* x on r: the fused loop also writes the r ring, and the set-up below rewrites every slot before the
+         * solve reads it (d_r from b - A x0, slot j in iteration j - 1) */
         double *xsave = c.d_x; c.d_x = cg->d_r;
         if (c.p2p) {
             OK(acgb200_p2p_begin(&pv->p2p, warmup, pv->stream));
@@ -2760,9 +2793,10 @@ int acgsolvercuda_solve_pipelined(
         }
         OK(iterate(&c, maxits, tol > 0, pipelined_iteration));
         if (c.fused) {
-            /* an even last update left p, x behind and r_{k+1} in d_r2; launched whatever the parity, so the
-             * launch count of a solve does not depend on where it stopped */
-            KL(acgb200_pcg_fused_finish(n, st, c.issued & 1, cg->d_r, pv->d_r2, cg->d_p, c.d_x, pv->stream));
+            /* a partial last group left p, x behind and its last r in the ring; launched wherever the solve
+             * stopped, so the launch count of a solve does not depend on it */
+            KL(acgb200_pcg_fused_finish(n, st, c.issued & 1, c.group, cg->d_r, pv->d_rring, pv->r_stride, cg->d_p,
+                                        c.d_x, pv->stream));
             c.launches += 1;
         }
         OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
@@ -2807,8 +2841,8 @@ int acgsolvercuda_solve_pipelined(
  *
  * In this library those three properties already hold for the loops behind
  * acgsolvercuda_solvempi / _solve_pipelined: scalars and the stopping test live
- * in the device control ring, the host only replays a captured two-iteration
- * graph and looks at the control word every few iterations, and between GPUs
+ * in the device control ring, the host only replays a captured graph of a few
+ * iterations and looks at the control word every few iterations, and between GPUs
  * the kernels themselves store halo values and reduction partials into the
  * peers' memory.  So with a null or NCCL communicator the device entry points
  * run those loops (same results, same report); what is *not* built is the fusion
@@ -3186,7 +3220,8 @@ int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info
     info->spmv_merge_threads = pv->plan.merge_threads; info->spmv_merge_grid = pv->plan.merge_grid;
     info->spmv_merge_stages = pv->plan.merge_stages;
     /* the bytes of what profile mode times as one product: the whole iteration on the fused path */
-    info->spmv_min_bytes = pv->last_fused ? acgb200_pcg_iteration_min_bytes(&pv->plan) : acgb200_spmv_min_bytes(&pv->plan);
+    info->spmv_min_bytes = pv->last_fused ? acgb200_pcg_iteration_min_bytes(&pv->plan, pv->last_group)
+                                          : acgb200_spmv_min_bytes(&pv->plan);
     info->spmv_slice_value_bytes = pv->plan.nslices > 0 ? pv->plan.sval_blocks * 32 * (int64_t) sizeof(double) : 0;
     info->spmv_slice_nnz = pv->plan.nslices > 0 ? pv->plan.slice_nnz : 0;
     info->spmv_symdiag_diagonals = pv->plan.symdiag_nd;
@@ -3199,5 +3234,6 @@ int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info
     info->cheb_degree = pv->last_cheb_degree; info->cheb_est_iterations = pv->last_cheb_est;
     info->cheb_breakdown = pv->last_cheb_breakdown;
     info->cheb_lmin = pv->last_cheb_lmin; info->cheb_lmax = pv->last_cheb_lmax;
+    info->pcg_group = pv->last_fused ? pv->last_group : 0;
     return ACG_SUCCESS;
 }

@@ -209,6 +209,9 @@ enum acgb200_spmvmode {
  * ------------------------------------------------------------------------ */
 struct acgb200_ctrl { int iter; int done; int pad0, pad1; };
 
+/* the largest group of iterations over which the fused pipelined CG defers its p and x updates */
+#define ACGB200_PCG_GROUP_MAX 16
+
 struct acgb200_devstate {
     struct acgb200_ctrl ctrl[4];     /* ring: kernel i of an iteration reads ctrl[i], writes ctrl[i+1 mod nk] */
     int maxits;
@@ -222,8 +225,10 @@ struct acgb200_devstate {
      * path, and on the fused path as a ring of three: iteration k reads slot k%3, adds into (k+1)%3 and
      * zeroes (k+2)%3, so its last kernel never adds into a slot it zeroes (DESIGN.md section 4a) */
     double gd_loc[3][2], gd[2][2];
-    double prev[2][3];               /* {gamma_{k-1}, alpha_{k-1}, beta_{k-1}} read by update k from slot k&1
-                                      * (beta: the fused path only, for the p and x updates it defers) */
+    double prev[2][2];               /* {gamma_{k-1}, alpha_{k-1}} read by update k from slot k&1 */
+    /* the fused path's {alpha_k, beta_k}, written by update k into slot k % ACGB200_PCG_GROUP_MAX and read by
+     * the catch-up update of k's group and by the finish (DESIGN.md section 4a) */
+    double ab[ACGB200_PCG_GROUP_MAX][2];
     /* setup-time reductions */
     double tmp_loc[2], tmp[2];
     unsigned int ticket;             /* spare (last-CTA detection on one GPU) */
@@ -362,15 +367,19 @@ int acgb200_pcg_update(int n, struct acgb200_devstate *st, int cin, int cout, in
  * or long rows: the covered rows' product and update in one kernel (spmv_symdiag_kernel with its PCG
  * epilogue), which reads the control word ctrl[cin] and writes ctrl[cin ^ 1].  With tiles, the tile kernel
  * (q = A w over the other rows) and their update run first and pass the word through ctrl[2] and ctrl[3].
- * w is read, w_{k+1} goes to w_next (another buffer: other rows still gather w); r_k is read from r and
- * r_{k+1} goes to r_next, which holds r_{k-1} on entry; z, t in place.  p and x are updated by odd
- * iterations only, for k-1 and k (DESIGN.md section 4a). */
+ * w is read, w_{k+1} goes to w_next (another buffer: other rows still gather w); z, t in place.  r_j lives
+ * in slot j % group of a ring: slot 0 is the solver's r, slot s > 0 is r_ring + (s - 1) r_stride.  r_k is
+ * read from r, slot k % group, and r_{k+1} goes to r_next, slot (k+1) % group.  p and x are updated by the
+ * catch-up iteration only, the last of each group, for the whole group (DESIGN.md section 4a). */
 struct acgb200_pcgargs {
     const struct acgb200_spmvplan *plan;
     const int *rowptr, *colidx; const double *a;    /* CSR of the tile rows */
     const double *w; double *w_next;
     double *q;                                      /* the tile rows' product */
     double *z, *t, *p, *r, *r_next, *x;
+    const double *r_ring; size_t r_stride;          /* slots 1 ... group - 1 of the r ring */
+    int group;                                      /* iterations per group, even, 2 ... ACGB200_PCG_GROUP_MAX */
+    int catchup;                                    /* 1: k % group == group - 1 */
     struct acgb200_devstate *st;
     int cin;                                        /* 0 or 1: the iteration's parity */
     int vec_evict_first;                            /* L2 policy of the fused kernel's vector streams */
@@ -383,16 +392,18 @@ struct acgb200_pcgargs {
 #define ACGB200_MULTI_LAUNCHER __attribute__((weak))
 #endif
 ACGB200_MULTI_LAUNCHER int acgb200_pcg_fused_launch(const struct acgb200_pcgargs *a, cudaStream_t stream);
-/* After the fused loop, whose final control word is ctrl[cfin]: if the last update was an even one, its p
- * and x updates, and its r_{k+1} moved from r2 into r; otherwise nothing.  Leaves p, x and r as the plain
- * recurrence does. */
-ACGB200_MULTI_LAUNCHER int acgb200_pcg_fused_finish(int n, const struct acgb200_devstate *st, int cfin, double *r,
-                                                    const double *r2, double *p, double *x, cudaStream_t stream);
+/* After the fused loop, whose final control word is ctrl[cfin]: if the updates done are not a multiple of
+ * the group, the p and x updates of the last, partial group, and the last r moved from its ring slot into r;
+ * otherwise nothing.  Leaves p, x and r as the plain recurrence does. */
+ACGB200_MULTI_LAUNCHER int acgb200_pcg_fused_finish(int n, const struct acgb200_devstate *st, int cfin, int group,
+                                                    double *r, const double *r_ring, size_t r_stride, double *p,
+                                                    double *x, cudaStream_t stream);
 /* the bytes the plain recurrence's fused launch moves (|D| elements + 96 per covered row), and those of a
- * whole fused iteration, averaged over an even and an odd one (the tile kernel's product, then per row of
- * the update 84 bytes in the slices and 92 in the tiles, DESIGN.md section 4a) */
+ * whole fused iteration, averaged over a group of `group` iterations (the tile kernel's product, then per
+ * row of the update 64 + (32 + 8 group) / group bytes in the slices and 8 more in the tiles, DESIGN.md
+ * section 4a) */
 int64_t acgb200_pcg_fused_min_bytes(const struct acgb200_spmvplan *plan);
-int64_t acgb200_pcg_iteration_min_bytes(const struct acgb200_spmvplan *plan);
+int64_t acgb200_pcg_iteration_min_bytes(const struct acgb200_spmvplan *plan, int group);
 
 /* the reference's public BLAS-1 building blocks (acg/cg-kernels-cuda.h:45-97; cgcuda.c wraps them) */
 int acgb200_helper_axpy(int op, int n, const double *num, const double *den, const double *x, double *y, cudaStream_t stream);

@@ -234,38 +234,64 @@ __device__ __forceinline__ PcgStep pcg_step(const acgb200_devstate *st, int iter
 }
 
 /*
- * Row i of update k, the fma chain of pcg_update_kernel: z=q+beta z; t=w+beta t; p=r+beta p; x+=alpha p;
- * r-=alpha t; w'=w-alpha z, w' into the other buffer; gamma'=(r,r), delta'=(w',r) accumulate in g2, d2.
- * p and x feed nothing but themselves, so they lag (DESIGN section 4a): an even k reads r_k from r, writes
- * r_{k+1} into r_next and leaves p and x alone; an odd k reads r_k from r and r_{k-1} from r_next, forms
- * p_{k-1} and p_k and both x updates -- the same FMAs in the same order -- and writes r_{k+1} over r_{k-1}.
- * lag (odd k only): {alpha_{k-1}, beta_{k-1}} in memory that the kernel does not write; st_vec clobbers
- * memory, so they are read per row rather than held in registers through the product loop.
+ * Row i of update k, the fma chain of pcg_update_kernel: z=q+beta z; t=w+beta t; r-=alpha t; w'=w-alpha z,
+ * w' into the other buffer; gamma'=(r,r), delta'=(w',r) accumulate in g2, d2.  r_k is read from r and
+ * r_{k+1} written to r_next.  p and x feed nothing but themselves, so they lag (DESIGN section 4a): their
+ * updates p=r+beta p; x+=alpha p are left to pcg_catchup once per group of iterations.
  */
-template <bool ODD>
-__device__ __forceinline__ void pcg_row(int i, double qi, double wi, double alpha, double beta, const double *lag,
-                                        double *__restrict__ z, double *__restrict__ t, double *__restrict__ p,
+__device__ __forceinline__ void pcg_row(int i, double qi, double wi, double alpha, double beta,
+                                        double *__restrict__ z, double *__restrict__ t,
                                         const double *__restrict__ r, double *__restrict__ r_next,
-                                        double *__restrict__ x, double *__restrict__ w_next, uint64_t pol,
-                                        double &g2, double &d2)
+                                        double *__restrict__ w_next, uint64_t pol, double &g2, double &d2)
 {
     const double zi = ld_vec(z + i, pol), ti = ld_vec(t + i, pol), ri = ld_vec(r + i, pol);
     const double zv = fma(beta, zi, qi);
     const double tv = fma(beta, ti, wi);
     const double rv = fma(-alpha, tv, ri);
     const double wv = fma(-alpha, zv, wi);
-    if (ODD) {
-        const double pi = ld_vec(p + i, pol), rp = ld_vec(r_next + i, pol), xi = ld_vec(x + i, pol);
-        const double pl = fma(lag[1], pi, rp);
-        const double pv = fma(beta, pl, ri);
-        st_vec(p + i, pv, pol);
-        st_vec(x + i, fma(alpha, pv, fma(lag[0], pl, xi)), pol);
-    }
     st_vec(z + i, zv, pol); st_vec(t + i, tv, pol);
     st_vec(r_next + i, rv, pol);
     st_vec(w_next + i, wv, pol);
     g2 = fma(rv, rv, g2);
     d2 = fma(wv, rv, d2);
+}
+
+/*
+ * Row i's p and x updates of a whole group j = k-m+1 ... k, run by the group's last iteration k before its
+ * pcg_row: p_j = r_j + beta_j p_{j-1}; x += alpha_j p_j, the FMAs of pcg_update_kernel in the same order.
+ * r_j lives in ring slot j % m: slot 0 (r_{k-m+1}) is the solver's r -- the slot pcg_row then overwrites
+ * with r_{k+1}, so the caller runs this first for the same rows on the same threads -- slot m-1 (r_k) is
+ * rk, and slot s in between is lag->ring + (s - 1) lag->stride.  ks: {alpha_j, beta_j} in order and lag,
+ * both in shared memory; the r's are loaded in batches of four ahead of their FMAs.
+ */
+struct PcgLag { const double *ring; size_t stride; int m; };
+
+__device__ __forceinline__ void pcg_catchup(int i, const double *ks, const PcgLag *lag, const double *r0,
+                                            const double *rk, double *__restrict__ p, double *__restrict__ x,
+                                            uint64_t pol)
+{
+    const int m = lag->m;
+    const size_t stride = lag->stride;
+    const double *ring = lag->ring + i;
+    double pv = ld_vec(p + i, pol), xv = ld_vec(x + i, pol);
+    for (int j0 = 0; j0 < m; j0 += 4) {
+        double rl[4];
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            const int j = j0 + u;
+            if (j < m) rl[u] = ld_vec(j == 0 ? r0 + i : j == m - 1 ? rk + i : ring + (size_t) (j - 1) * stride, pol);
+        }
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            const int j = j0 + u;
+            if (j < m) {
+                pv = fma(ks[2 * j + 1], pv, rl[u]);
+                xv = fma(ks[2 * j], pv, xv);
+            }
+        }
+    }
+    st_vec(p + i, pv, pol);
+    st_vec(x + i, xv, pol);
 }
 
 /* ------------------------------------------------------------------------ */
@@ -816,8 +842,12 @@ struct SymdiagParams {
     acgb200_devstate *st;
     int housekeeping;
     /* pipelined-CG epilogue (PCG): x above is w_k; z, t, p, xs updated in place, w_{k+1} into w_next, r_k
-     * read from r and r_{k+1} written to r_next (pcg_row) */
+     * read from r and r_{k+1} written to r_next; the catch-up form reads the group's lagged r's from r_next
+     * and r_ring (pcg_catchup) */
     double *z, *t, *p, *r, *r_next, *xs, *w_next;
+    const double *r_ring;
+    size_t r_stride;
+    int group;
     int vec_evict_first;
 };
 
@@ -838,7 +868,8 @@ struct SymdiagParams {
  * and goes straight into the update (pcg_row) instead of to memory; the kernel is the iteration's last, so
  * block 0 advances the control word and zeroes ring slot (k+2) % 3 while every CTA adds into (k+1) % 3.
  * A met convergence test returns before the product.  At most 40 registers: 12 CTAs of 128 threads.
- * ODD: the parity of k, which decides whether the row also catches up on p and x (pcg_row).
+ * CATCH: k is the last of its group of P.group iterations, so a pass over the same rows before the product
+ * catches up on p and x for the group (pcg_catchup).
  *
  * V: double reads the fp64 diagonals (hval); uint8_t reads one code per element (hcode) and decodes it from
  * a copy of the value table in shared memory just before the FMAs -- the same double, bit for bit, so the
@@ -893,14 +924,14 @@ __device__ __forceinline__ double symdiag_row_sum(const SymdiagParams &P, const 
     return sum;
 }
 
-template <int UB, int T, bool PCG, typename V, typename X = double, bool ODD = false>
+template <int UB, int T, bool PCG, typename V, typename X = double, bool CATCH = false>
 __global__ void __launch_bounds__(T, PCG ? 1536 / T : 0)
 spmv_symdiag_kernel(const SymdiagParams P)
 {
     constexpr bool CODED = std::is_same<V, uint8_t>::value;
     constexpr bool F32 = std::is_same<X, float>::value;
     static_assert(!(F32 && PCG), "the fused pipelined-CG epilogue is fp64 only");
-    static_assert(PCG || !ODD, "parity only selects the fused epilogue's form");
+    static_assert(PCG || !CATCH, "the catch-up form belongs to the fused epilogue");
     __shared__ int2 tab_s[ACGB200_SYMDIAG_MAX];
     __shared__ double vtab_s[CODED ? 256 : 1];
     __shared__ double red[T / 32];
@@ -918,7 +949,9 @@ spmv_symdiag_kernel(const SymdiagParams P)
                 if (k.conv) { c.done = 1; P.st->final_rr = k.gamma; }
                 else {
                     c.iter = gate.iter + 1;
-                    P.st->prev[s ^ 1][0] = k.gamma; P.st->prev[s ^ 1][1] = k.alpha; P.st->prev[s ^ 1][2] = k.beta;
+                    P.st->prev[s ^ 1][0] = k.gamma; P.st->prev[s ^ 1][1] = k.alpha;
+                    double *ab = P.st->ab[gate.iter % ACGB200_PCG_GROUP_MAX];
+                    ab[0] = k.alpha; ab[1] = k.beta;
                 }
             }
             *P.ctrl_out = c;
@@ -933,10 +966,18 @@ spmv_symdiag_kernel(const SymdiagParams P)
         }
     }
     if (!gate.active) return;
-    /* ODD: {alpha_k, beta_k, alpha_{k-1}, beta_{k-1}} for pcg_row, from shared memory rather than registers
-     * (the second pair would make the fp64 loops spill); prev[1] is written by even iterations only */
-    __shared__ double ks_s[ODD ? 4 : 1];
-    if (ODD && tid == 0) { ks_s[0] = k.alpha; ks_s[1] = k.beta; ks_s[2] = P.st->prev[1][1]; ks_s[3] = P.st->prev[1][2]; }
+    /* CATCH: {alpha_j, beta_j} for j = k-m+1 ... k and the ring for pcg_catchup, in shared memory; this kernel
+     * writes only slot k of the device ring */
+    __shared__ double ks_s[CATCH ? 2 * ACGB200_PCG_GROUP_MAX : 1];
+    __shared__ PcgLag lag_s;
+    if (CATCH) {
+        const int m = P.group;
+        if (tid < 2 * (m - 1)) ks_s[tid] = P.st->ab[(gate.iter - (m - 1) + (tid >> 1)) % ACGB200_PCG_GROUP_MAX][tid & 1];
+        if (tid == 0) {
+            ks_s[2 * m - 2] = k.alpha; ks_s[2 * m - 1] = k.beta;
+            lag_s.ring = P.r_ring; lag_s.stride = P.r_stride; lag_s.m = m;
+        }
+    }
     if (tid < P.no) tab_s[tid] = make_int2(P.tab[tid].voff, P.tab[tid].coff);
     if (CODED) for (int i = tid; i < P.ncodes; i += T) vtab_s[i] = __ldg(P.vtab + i);
     __syncthreads();
@@ -951,13 +992,18 @@ spmv_symdiag_kernel(const SymdiagParams P)
     double dot = 0.0, dot2 = 0.0;
     /* the vector streams of the update pass through L2 once: see the measurements in DESIGN section 4a */
     const uint64_t vpol = PCG ? (P.vec_evict_first ? l2_policy_evict_first() : l2_policy_evict_normal()) : 0;
+    if (CATCH) {
+        /* the group's p and x, in a pass of their own so that the product loop keeps the plain form's
+         * registers; the same rows on the same threads as that loop, which overwrites r_{k-m+1} */
+        for (int s = warp; s < P.nslices; s += nwarps)
+            pcg_catchup(__ldg(&P.slices[s].row0) + lane, ks_s, &lag_s, P.r_next, P.r, P.p, P.xs, vpol);
+    }
     for (int s = warp; s < P.nslices; s += nwarps) {
         const int row = __ldg(&P.slices[s].row0) + lane;
         const double sum = symdiag_row_sum<UB, V, X>(P, tab_s, vtab_s, row, pol, cmax, L);
         if (PCG) {
             /* w_i was gathered by this row a moment ago: an L1 hit, not a third stream */
-            pcg_row<ODD>(row, sum, __ldg(P.x + row), ODD ? ks_s[0] : k.alpha, ODD ? ks_s[1] : k.beta, ks_s + 2,
-                         P.z, P.t, P.p, P.r, P.r_next, P.xs, P.w_next, vpol, dot, dot2);
+            pcg_row(row, sum, __ldg(P.x + row), k.alpha, k.beta, P.z, P.t, P.r, P.r_next, P.w_next, vpol, dot, dot2);
         } else if (F32) {
             const X ys = (X) sum;
             sd_vec<X>(P.y)[row] = ys;
@@ -1740,27 +1786,40 @@ pcg_update_kernel(int n, acgb200_devstate *st, int cin, int cout, int multi, acg
  * row ranges of the tile plan, one CTA per tile and trip.  Adds into the same ring slot as the fused kernel,
  * which runs after it and advances the control word; this one only forwards it. */
 #define PCG_TAIL_THREADS 128
-template <bool ODD>
+template <bool CATCH>
 __global__ void __launch_bounds__(PCG_TAIL_THREADS)
 pcg_tail_update_kernel(const acgb200_tile *__restrict__ tiles, int ntiles, acgb200_devstate *st,
                        const acgb200_ctrl *cin, acgb200_ctrl *cout, const double *__restrict__ q,
                        const double *__restrict__ w, double *__restrict__ w_next, double *__restrict__ z,
                        double *__restrict__ t, double *__restrict__ p, const double *__restrict__ r,
-                       double *__restrict__ r_next, double *__restrict__ x)
+                       double *__restrict__ r_next, const double *__restrict__ r_ring, size_t r_stride, int m,
+                       double *__restrict__ x)
 {
     __shared__ double red[PCG_TAIL_THREADS / 32];
+    __shared__ double ks_s[CATCH ? 2 * ACGB200_PCG_GROUP_MAX : 1];
+    __shared__ PcgLag lag_s;
     pdl_prologue();
     const Gate g = gate_read(cin, st);
     if (blockIdx.x == 0 && threadIdx.x == 0) *cout = *cin;
     if (!g.active) return;
     const PcgStep k = pcg_step(st, g.iter);
     if (k.conv) return;
+    /* CATCH: the group's {alpha_j, beta_j} and the ring, as in spmv_symdiag_kernel */
+    if (CATCH && threadIdx.x < 2 * (m - 1))
+        ks_s[threadIdx.x] = st->ab[(g.iter - (m - 1) + (int) (threadIdx.x >> 1)) % ACGB200_PCG_GROUP_MAX][threadIdx.x & 1];
+    if (CATCH && threadIdx.x == 0) {
+        ks_s[2 * m - 2] = k.alpha; ks_s[2 * m - 1] = k.beta;
+        lag_s.ring = r_ring; lag_s.stride = r_stride; lag_s.m = m;
+    }
+    if (CATCH) __syncthreads();
     const uint64_t pol = l2_policy_evict_normal();
     double g2 = 0.0, d2 = 0.0;
     for (int b = blockIdx.x; b < ntiles; b += gridDim.x) {
         const acgb200_tile tl = tiles[b];
-        for (int i = tl.row_begin + (int) threadIdx.x; i < tl.row_begin + tl.nrows; i += PCG_TAIL_THREADS)
-            pcg_row<ODD>(i, q[i], w[i], k.alpha, k.beta, &st->prev[1][1], z, t, p, r, r_next, x, w_next, pol, g2, d2);
+        for (int i = tl.row_begin + (int) threadIdx.x; i < tl.row_begin + tl.nrows; i += PCG_TAIL_THREADS) {
+            if (CATCH) pcg_catchup(i, ks_s, &lag_s, r_next, r, p, x, pol);
+            pcg_row(i, q[i], w[i], k.alpha, k.beta, z, t, r, r_next, w_next, pol, g2, d2);
+        }
     }
     g2 = block_sum(g2, red);
     d2 = block_sum(d2, red);
@@ -1771,21 +1830,26 @@ pcg_tail_update_kernel(const acgb200_tile *__restrict__ tiles, int ntiles, acgb2
     }
 }
 
-/* Fused pipelined CG, after the loop: the final control word counts the updates m.  If m is odd, the last
- * one (m - 1, even) left its p and x updates to an iteration that did not run, and its r_m sits in r2: form
- * p_{m-1} = r_{m-1} + beta_{m-1} p and x += alpha_{m-1} p_{m-1} (pcg_row's FMAs), and move r_m into r. */
+/* Fused pipelined CG, after the loop: the final control word counts the updates it.  If it is not a multiple
+ * of the group m, updates g = m floor(it/m) ... it - 1 left their p and x updates to a catch-up iteration that
+ * did not run, and r_it sits in ring slot it - g: form p_j = r_j + beta_j p and x += alpha_j p_j for those j
+ * (pcg_row's FMAs; r_g is r itself, the others are in the ring), and move r_it into r. */
 __global__ void __launch_bounds__(BLAS1_THREADS)
-pcg_fused_finish_kernel(int n, const acgb200_devstate *st, int cfin, double *__restrict__ r,
-                        const double *__restrict__ r2, double *__restrict__ p, double *__restrict__ x)
+pcg_fused_finish_kernel(int n, const acgb200_devstate *st, int cfin, int m, double *__restrict__ r,
+                        const double *__restrict__ ring, size_t stride, double *__restrict__ p, double *__restrict__ x)
 {
-    const int m = st->ctrl[cfin].iter;
-    if (!(m & 1)) return;
-    const double alpha = st->prev[1][1], beta = st->prev[1][2];
+    const int it = st->ctrl[cfin].iter, lag = it % m, g = it - lag;
+    if (lag == 0) return;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const double pv = fma(beta, p[i], r[i]);
+        double pv = p[i], xv = x[i];
+        for (int j = 0; j < lag; j++) {
+            const double *ab = st->ab[(g + j) % ACGB200_PCG_GROUP_MAX];
+            pv = fma(ab[1], pv, j ? ring[(size_t) (j - 1) * stride + i] : r[i]);
+            xv = fma(ab[0], pv, xv);
+        }
         p[i] = pv;
-        x[i] = fma(alpha, pv, x[i]);
-        r[i] = r2[i];
+        x[i] = xv;
+        r[i] = ring[(size_t) (lag - 1) * stride + i];
     }
 }
 
@@ -2981,11 +3045,11 @@ static slice_fn slice_variant(int UB, int T, int EXC)
 typedef void (*symdiag_fn)(const SymdiagParams);
 
 /* the mirrored-diagonal kernel for exactly the (UB, T) pairs of slice_variant; pcg: with the fused
- * pipelined-CG epilogue, odd: its form for odd iterations; coded: reading one-byte codes (the plan's
- * symdiag_codes > 0) */
-static symdiag_fn symdiag_variant(int UB, int T, bool pcg, bool odd, bool coded)
+ * pipelined-CG epilogue, catchup: its form for the last iteration of a group; coded: reading one-byte codes
+ * (the plan's symdiag_codes > 0) */
+static symdiag_fn symdiag_variant(int UB, int T, bool pcg, bool catchup, bool coded)
 {
-#define V(u, t, c) (pcg ? (odd ? spmv_symdiag_kernel<u, t, true, c, double, true> : spmv_symdiag_kernel<u, t, true, c>) \
+#define V(u, t, c) (pcg ? (catchup ? spmv_symdiag_kernel<u, t, true, c, double, true> : spmv_symdiag_kernel<u, t, true, c>) \
                         : spmv_symdiag_kernel<u, t, false, c>)
 #define X(u, t) if (UB == u && T == t) return coded ? V(u, t, uint8_t) : V(u, t, double);
     X(5, 128) X(7, 128) X(8, 128) X(9, 128) X(7, 256) X(8, 256) X(9, 256)
@@ -2994,9 +3058,9 @@ static symdiag_fn symdiag_variant(int UB, int T, bool pcg, bool odd, bool coded)
     return NULL;
 }
 
-static symdiag_fn symdiag_variant(const acgb200_spmvplan *pl, bool pcg, bool odd = false)
+static symdiag_fn symdiag_variant(const acgb200_spmvplan *pl, bool pcg, bool catchup = false)
 {
-    return symdiag_variant(pl->slice_ub, pl->slice_threads, pcg, odd, pl->symdiag_codes > 0);
+    return symdiag_variant(pl->slice_ub, pl->slice_threads, pcg, catchup, pl->symdiag_codes > 0);
 }
 
 /* the float-vector product of the mixed-precision solve, for the same (UB, T) pairs */
@@ -3119,8 +3183,8 @@ extern "C" int acgb200_spmv_configure(acgb200_spmvplan *pl)
         pl->slice_grid = (int) (sgrid < 1 ? 1 : sgrid);
         pl->pcg_grid = 0;
         if (pl->symdiag_nd > 0) {
-            /* the fused pipelined-CG kernel: the same grid, unless the registers of either parity's form
-             * allow fewer CTAs */
+            /* the fused pipelined-CG kernel: the same grid, unless the registers of its plain or its catch-up
+             * form allow fewer CTAs */
             int fper = 0, oper = 0;
             err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fper, (const void *) symdiag_variant(pl, true, false),
                                                                 pl->slice_threads, 0);
@@ -3331,11 +3395,12 @@ extern "C" int acgb200_pcg_fused_launch(const acgb200_pcgargs *a, cudaStream_t s
         long long grid = pl->ntiles;
         const long long cap = (long long) acgb200_num_sms() * 8;
         if (grid > cap) grid = cap;
-        const cudaError_t le = launch_chain(a->cin ? pcg_tail_update_kernel<true> : pcg_tail_update_kernel<false>,
+        const cudaError_t le = launch_chain(a->catchup ? pcg_tail_update_kernel<true> : pcg_tail_update_kernel<false>,
                                             (int) grid, PCG_TAIL_THREADS, 0, stream,
                                             (const acgb200_tile *) pl->d_tiles, pl->ntiles, a->st,
                                             (const acgb200_ctrl *) &ctrl[2], &ctrl[3], (const double *) a->q, a->w,
-                                            a->w_next, a->z, a->t, a->p, (const double *) a->r, a->r_next, a->x);
+                                            a->w_next, a->z, a->t, a->p, (const double *) a->r, a->r_next,
+                                            (const double *) a->r_ring, a->r_stride, a->group, a->x);
         if (le) return (int) le;
         fin = 3;
     }
@@ -3345,19 +3410,20 @@ extern "C" int acgb200_pcg_fused_launch(const acgb200_pcgargs *a, cudaStream_t s
     S.x = a->w; S.mode = SPMV_Y_AX;
     S.ctrl_in = &ctrl[fin]; S.ctrl_out = &ctrl[cout]; S.st = a->st;
     S.z = a->z; S.t = a->t; S.p = a->p; S.r = a->r; S.r_next = a->r_next; S.xs = a->x; S.w_next = a->w_next;
+    S.r_ring = a->r_ring; S.r_stride = a->r_stride; S.group = a->group;
     S.vec_evict_first = a->vec_evict_first;
-    const cudaError_t le = launch_chain(symdiag_variant(pl, true, a->cin != 0), pl->pcg_grid, pl->slice_threads,
+    const cudaError_t le = launch_chain(symdiag_variant(pl, true, a->catchup != 0), pl->pcg_grid, pl->slice_threads,
                                         (size_t) 0, stream, S);
     if (le) return (int) le;
     return (int) cudaGetLastError();
 }
 
-extern "C" int acgb200_pcg_fused_finish(int n, const acgb200_devstate *st, int cfin, double *r, const double *r2,
-                                        double *p, double *x, cudaStream_t stream)
+extern "C" int acgb200_pcg_fused_finish(int n, const acgb200_devstate *st, int cfin, int group, double *r,
+                                        const double *r_ring, size_t r_stride, double *p, double *x, cudaStream_t stream)
 {
     static int occ = 0;
     pcg_fused_finish_kernel<<<blas1_grid(n, (const void *) pcg_fused_finish_kernel, &occ), BLAS1_THREADS, 0, stream>>>(
-        n, st, cfin, r, r2, p, x);
+        n, st, cfin, group, r, r_ring, r_stride, p, x);
     return (int) cudaGetLastError();
 }
 

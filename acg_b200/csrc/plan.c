@@ -30,13 +30,16 @@ int64_t acgb200_pcg_fused_min_bytes(const struct acgb200_spmvplan *pl)
     return (int64_t) pl->slice_rows * (symdiag_elem_bytes(pl) * pl->symdiag_nd + 96);
 }
 
-/* the whole fused iteration as it runs, p and x updated every second iteration: the tile kernel's product,
- * then per row the mean of an even and an odd update.  Covered rows: w_i, z t r read, z t r w' written
- * (64), and w_i, z t r r_prev p x read, z t p x r w' written (104).  Tile rows: q_i read on top (72, 112). */
-int64_t acgb200_pcg_iteration_min_bytes(const struct acgb200_spmvplan *pl)
+/* the whole fused iteration as it runs, p and x updated once per group of m iterations: the tile kernel's
+ * product, then per row the mean over a group.  Covered rows: w_i, z t r read, z t r w' written (64) in
+ * every iteration, and in the group's last one a pass that reads the group's m r's and p x and writes p x,
+ * so 64 + (32 + 8 m) / m = (72 m + 32) / m on average.  Tile rows: q_i read on top. */
+int64_t acgb200_pcg_iteration_min_bytes(const struct acgb200_spmvplan *pl, int m)
 {
     const int64_t tnnz = pl->nnz - pl->slice_nnz, trows = pl->nrows - pl->slice_rows;
-    return tnnz * 12 + trows * (20 + 92) + (int64_t) pl->slice_rows * (symdiag_elem_bytes(pl) * pl->symdiag_nd + 84);
+    return tnnz * 12 + trows * 20 + (trows * (80 * (int64_t) m + 32)) / m
+           + (int64_t) pl->slice_rows * symdiag_elem_bytes(pl) * pl->symdiag_nd
+           + ((int64_t) pl->slice_rows * (72 * (int64_t) m + 32)) / m;
 }
 
 /*

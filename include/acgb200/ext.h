@@ -25,8 +25,9 @@ extern "C" {
  * default -1: merge-path tiles when the row lengths are irregular, mergeplan.c; "merge_items", "merge_threads",
  * "merge_max_ctas"), "pcg_fused" (1/0, default 1: pipelined CG on one GPU runs each iteration's product and
  * vector update in one kernel when the plan has mirrored diagonals and no merge tiles, medium or long rows;
- * "pcg_evict_first" 1/0 the L2 policy of its vector streams), "spmv_medium", "graph"
- * (0/1: replay iteration pairs as CUDA graphs), "redstream" (0/1: pipelined
+ * "pcg_evict_first" 1/0 the L2 policy of its vector streams; "pcg_group" 2/4/8/16, default 16: it updates p
+ * and x once per that many iterations, other values are refused), "spmv_medium", "graph"
+ * (0/1: replay groups of iterations as CUDA graphs), "redstream" (0/1: pipelined
  * allreduce on its own stream and communicator; read at acgsolvercuda_init).  Environment variables ACGB200_<KEY> set the
  * same values at first use. */
 ACG_API int acgb200_set_option(const char *key, int value);
@@ -230,6 +231,8 @@ struct acgb200_info {
      * ran), 1 if a breakdown ended it, and the interval [cheb_lmin, cheb_lmax] used (0, 0: none) */
     int cheb_degree, cheb_est_iterations, cheb_breakdown;
     double cheb_lmin, cheb_lmax;
+    int pcg_group;                              /* the group of the last solve if it was fused pipelined CG (option
+                                                   "pcg_group"), 0 otherwise */
 };
 ACG_API int acgsolvercuda_info(const struct acgsolvercuda *cg, struct acgb200_info *info);
 

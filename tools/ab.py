@@ -23,7 +23,8 @@ import numpy as np          # noqa: E402
 DEFAULTS = dict(profile=0, spmv_lanes=0, spmv_nnz_cap=0, spmv_rows_cap=0, spmv_stages=0, spmv_threads=0,
                 spmv_unroll=0, spmv_max_ctas=0, graph=1, redstream=1, p2p=1, p2p_fuse=1, blas1_ctas=0, pdl=0,
                 spmv_medium=0, spmv_merge=-1, merge_items=0, merge_threads=0, merge_stages=0, merge_max_ctas=0, spmv_slices=1, slice_ub=0, slice_threads=0, slice_max_ctas=0,
-                spmv_symdiag=1, symdiag_evict_first=0, symdiag_codes=1, pcg_fused=1, pcg_evict_first=1)
+                spmv_symdiag=1, symdiag_evict_first=0, symdiag_codes=1, pcg_fused=1, pcg_evict_first=1,
+                pcg_group=16)
 
 VARIANTS = {
     "base": {},
@@ -53,6 +54,8 @@ VARIANTS = {
     "nofuse": {"pcg_fused": 0}, "fuse_en": {"pcg_evict_first": 0},
     # the mirrored diagonals as fp64 values even where one-byte codes into a value table would do
     "nocodes": {"symdiag_codes": 0},
+    # the fused pipelined-CG iteration's group: p and x updated once per 2, 4, 8 or 16 iterations
+    "g2": {"pcg_group": 2}, "g4": {"pcg_group": 4}, "g8": {"pcg_group": 8}, "g16": {"pcg_group": 16},
 }
 
 
