@@ -166,7 +166,7 @@ EXPORTS = [
     "acgsolvercuda_init_constants", "acgsolvercuda_alpha", "acgsolvercuda_beta", "acgsolvercuda_daxpy_alpha",
     "acgsolvercuda_daxpy_minus_alpha", "acgsolvercuda_daypx_beta", "acgsolvercuda_pipelined_daxpy_fused",
     "acgsolvercuda_fwrite",
-    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_solve_multi", "acgsolvercuda_spmm_mode", "acgsolvercuda_solve_shifted", "acgsolvercuda_solve_minres", "acgsolvercuda_solve_mixed", "acgsolvercuda_spmv_f32", "acgsolvercuda_solve_chebyshev", "acgb200_cheb_interval_host", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
+    "acgb200_set_option", "acgsolvercuda_spmv", "acgsolvercuda_spmv_ghost", "acgsolvercuda_spmv_mode", "acgsolvercuda_solve_multi", "acgsolvercuda_spmm_mode", "acgsolvercuda_solve_shifted", "acgsolvercuda_solve_minres", "acgsolvercuda_solve_mixed", "acgsolvercuda_spmv_f32", "acgsolvercuda_solve_chebyshev", "acgsolvercuda_update_values", "acgb200_cheb_interval_host", "acgsolvercuda_info", "acgb200_sizeof", "acgb200_have_mpi",
     "acgb200_nccl_unique_id", "acgb200_comm_init_rank", "acgb200_comm_destroy",
     "acgb200_host_register", "acgb200_host_unregister", "acgb200_spmv_plan_host", "acgb200_spmv_plan_host2", "acgb200_slices_host", "acgb200_symdiag_host", "acgb200_merge_plan_host", "acgb200_p2p_inverse_map", "acgb200_patterns_host", "acgb200_stencil_part",
     "acgb200_mtx_info", "acgb200_mtx_read", "acgb200_mtx_read_part", "acgb200_comm_matrix_row", "acgb200_partition_rows_grid", "acgb200_grid_factors", "acgb200_rmat_spd",
@@ -260,6 +260,7 @@ def lib() -> C.CDLL:
                                             C.c_double, C.c_double, C.c_int, P(C.c_int)]
     f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
     L.acgsolvercuda_spmv_f32.argtypes = [P(acgsolvercuda), f32p, f32p, P(C.c_double)]
+    L.acgsolvercuda_update_values.argtypes = [P(acgsolvercuda), P(acgsymcsrmatrix), P(C.c_int)]
     L.acgsolvercuda_info.argtypes = [P(acgsolvercuda), P(acgb200_info)]
     L.acgb200_set_option.argtypes = [C.c_char_p, C.c_int]
     L.acgb200_nccl_unique_id.argtypes = [C.c_void_p]
@@ -883,6 +884,16 @@ class SolverCuda:
         dots = (C.c_double * k)()
         _check(lib().acgsolvercuda_spmm_mode(C.byref(self.c), int(mode), k, X, bp, Y, dots), "acgsolvercuda_spmm_mode")
         return Y, np.array(dots[:], np.float64)
+
+    def update_values(self, A: SymCsrMatrix):
+        """acgsolvercuda_update_values: take A's values (full storage if A has it, else its packed triangle)
+        into the solver, keeping every plan built from the pattern.  A must have the partition and pattern of
+        the matrix the solver was built on; anything else raises with the solver unchanged.  Solves then take
+        A as their matrix."""
+        err = C.c_int(0)
+        _check(lib().acgsolvercuda_update_values(C.byref(self.c), C.byref(A.c), C.byref(err)),
+               "acgsolvercuda_update_values", err.value)
+        self.A = A
 
     def info(self) -> dict:
         inf = acgb200_info()

@@ -172,7 +172,7 @@ struct priv {
     struct acgb200_devstate *d_st;
     struct acgb200_ctrl *h_ctrl;        /* pinned, 2 poll slots */
     struct acgb200_devstate *h_st;      /* pinned scratch for state upload / readback */
-    int nowned, ninner, nborder, nghost, borderoff, nvec;
+    int nrows, nowned, ninner, nborder, nghost, borderoff, nvec;
     int64_t fnnz, onnz;
     int device_expanded;                /* the full storage was built on the device (the host matrix has none) */
     cudaStream_t stream, commstream, redstream;
@@ -634,7 +634,31 @@ static int upload_block(int **d_col, double **d_val, const acgidx_t *col, const 
     return ACG_SUCCESS;
 }
 
+/* The device full storage of A as the solver takes it: A's own full storage when it has one, else the packed
+ * triangle mirrored on the device (expand.cu) into the arrays acgsymcsrmatrix_dsymv_init(A, 0) would have made.
+ * Columns 0-based either way; padded for the tile kernel's bulk copies.  Nothing is left allocated on failure. */
+static int upload_matrix(const struct acgsymcsrmatrix *A, struct acgb200_expanded *ex, cudaStream_t stream, int *errcode)
+{
+    if (!A->frowptr) return acgb200_expand_upload(A, 0.0, 8, 16, ex, stream, errcode);
+    memset(ex, 0, sizeof(*ex));
+    int err = upload_rowptr(&ex->d_rowptr, A->frowptr, A->nprows, 8, errcode);
+    if (!err) err = upload_block(&ex->d_colidx, &ex->d_a, A->fcolidx, A->fa, A->fnpnzs, A->rowidxbase, 16, errcode);
+    if (!err) err = upload_rowptr(&ex->d_orowptr, A->orowptr, (int64_t) A->nborderrows + A->nghostrows, 8, errcode);
+    if (!err) err = upload_block(&ex->d_ocolidx, &ex->d_oa, A->ocolidx, A->oa, A->onpnzs, A->rowidxbase, 16, errcode);
+    if (err) { acgb200_expanded_free(ex); return err; }
+    ex->fnnz = A->fnpnzs; ex->onnz = A->onpnzs;
+    return ACG_SUCCESS;
+}
+
+/* A has full storage, or the packed triangle to build it from */
+static int matrix_usable(const struct acgsymcsrmatrix *A)
+{
+    if (!A->frowptr && !A->rowptr) return 0;
+    return !A->frowptr || (A->fcolidx && A->fa);
+}
+
 static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, const struct acgcomm *comm);
+static int fill_values(struct acgsolvercuda *cg, struct priv *pv, int *errcode);
 
 int acgsolvercuda_init(
     struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A,
@@ -644,8 +668,7 @@ int acgsolvercuda_init(
     memset(cg, 0, sizeof(*cg));
     cfg_load();
     /* without full storage (no acgsymcsrmatrix_dsymv_init call) the packed triangle is expanded on the device */
-    if (!A->frowptr && !A->rowptr) return ACG_ERR_INVALID_VALUE;
-    if (A->frowptr && (!A->fcolidx || !A->fa)) return ACG_ERR_INVALID_VALUE;
+    if (!matrix_usable(A)) return ACG_ERR_INVALID_VALUE;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) return ACG_ERR_CUDA;   /* no CPU fallback */
     int err = init_impl(cg, A, comm);
@@ -729,7 +752,7 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
     }
 
     pv->commsize = commsize;
-    pv->nowned = A->nownedrows; pv->ninner = A->ninnerrows; pv->nborder = A->nborderrows;
+    pv->nrows = A->nrows; pv->nowned = A->nownedrows; pv->ninner = A->ninnerrows; pv->nborder = A->nborderrows;
     pv->nghost = A->nghostrows; pv->borderoff = A->borderrowoffset;
     pv->nvec = cg->r.num_nonzeros;
 
@@ -747,26 +770,19 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
     CU(cudaMalloc((void **) &cg->d_t, vbytes)); CU(cudaMemset(cg->d_t, 0, vbytes));
 
     /* local block (rows [0,nowned) of the full storage) and border x ghost block */
+    struct acgb200_expanded ex;
+    OK(upload_matrix(A, &ex, pv->stream, errcode));
+    cg->d_rowptr = ex.d_rowptr; cg->d_colidx = ex.d_colidx; cg->d_a = ex.d_a;
+    cg->d_orowptr = ex.d_orowptr; cg->d_ocolidx = ex.d_ocolidx; cg->d_oa = ex.d_oa;
+    pv->fnnz = ex.fnnz; pv->onnz = ex.onnz;
     const int64_t *frp = A->frowptr;          /* host row pointers / columns of the local block, for the plans */
     const acgidx_t *fcol = A->fcolidx;
     int64_t *frp_tmp = NULL;
     acgidx_t *fcol_tmp = NULL;
-    if (A->frowptr) {
-        OK(upload_rowptr(&cg->d_rowptr, A->frowptr, A->nprows, 8, errcode));
-        OK(upload_block(&cg->d_colidx, &cg->d_a, A->fcolidx, A->fa, A->fnpnzs, A->rowidxbase, 16, errcode));
-        OK(upload_rowptr(&cg->d_orowptr, A->orowptr, (int64_t) A->nborderrows + A->nghostrows, 8, errcode));
-        OK(upload_block(&cg->d_ocolidx, &cg->d_oa, A->ocolidx, A->oa, A->onpnzs, A->rowidxbase, 16, errcode));
-        pv->fnnz = A->fnpnzs; pv->onnz = A->onpnzs;
-    } else {
-        /* the caller did not build full storage: upload the packed triangle (half the bytes) and mirror it
-         * on the device (expand.cu) -- the arrays are those acgsymcsrmatrix_dsymv_init(A, 0) would have made */
-        struct acgb200_expanded ex;
-        OK(acgb200_expand_upload(A, 0.0, 8, 16, &ex, pv->stream, errcode));
-        cg->d_rowptr = ex.d_rowptr; cg->d_colidx = ex.d_colidx; cg->d_a = ex.d_a;
-        cg->d_orowptr = ex.d_orowptr; cg->d_ocolidx = ex.d_ocolidx; cg->d_oa = ex.d_oa;
-        pv->fnnz = ex.fnnz; pv->onnz = ex.onnz;
+    if (!A->frowptr) {
+        /* the caller did not build full storage: the packed triangle (half the bytes) was mirrored on the device,
+         * and the planners work on the host -- row pointers always, columns only for the pattern dictionary */
         pv->device_expanded = 1;
-        /* the planners work on the host: row pointers always, columns only for the pattern dictionary */
         int *t = malloc(((size_t) A->nprows + 1) * sizeof(*t));
         frp_tmp = malloc(((size_t) A->nprows + 1) * sizeof(*frp_tmp));
         if (!t || !frp_tmp) { free(t); free(frp_tmp); return ACG_ERR_ERRNO; }
@@ -797,7 +813,6 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
     if (cfg.spmv_threads > 0) pv->plan.threads = cfg.spmv_threads;
     if (cfg.spmv_unroll > 0) pv->plan.unroll = cfg.spmv_unroll;
     pv->plan.med_thr = cfg.spmv_medium;
-    int slice_domlen = 0;
     {
         struct acgb200_patterns pat;
         struct acgb200_sliceplan sp;
@@ -832,12 +847,13 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
         }
         acgb200_mergeplan_free(&mp);
         if (!err && pv->plan.nslices > 0) {
-            slice_domlen = sp.domlen;
+            pv->plan.slice_domlen = sp.domlen;
+            pv->plan.slice_ub_opt = cfg.slice_ub;
             pv->plan.slice_threads = cfg.slice_threads > 0 ? cfg.slice_threads : 128;
             pv->plan.slice_max_ctas = cfg.slice_max_ctas;
         }
         if (!err && pv->plan.nslices > 0 && cfg.spmv_symdiag) {
-            /* mirrored diagonals: planned here, stored and checked by acgb200_slices_fill below */
+            /* mirrored diagonals: planned here, stored and checked by fill_values */
             struct acgb200_symdiag sd;
             err = acgb200_symdiag_plan(A->nownedrows, &sp, &pat, &sd);
             if (!err && sd.reason == SYMDIAG_OK) {
@@ -846,15 +862,7 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
                 memcpy(pl->symdiag_d, sd.d, (size_t) sd.nd * sizeof(int));
                 pl->symdiag_nd = sd.nd; pl->symdiag_no = sd.no;
                 pl->symdiag_evict_first = cfg.symdiag_evict_first;
-                pl->symdiag_colidx = cg->d_colidx;
-                cudaError_t e = cudaMalloc((void **) &pl->d_hval, (size_t) sd.nd * (size_t) pl->symdiag_stride * sizeof(double));
-                if (!e) e = cudaMalloc((void **) &pl->d_symdiag_bad, sizeof(int));
-                /* "failed" until the device check has run and passed */
-                if (!e) { const int one = 1; e = cudaMemcpy(pl->d_symdiag_bad, &one, sizeof(int), cudaMemcpyHostToDevice); }
-                /* room for the coded layout, which the fill builds and checks too */
-                if (!e && cfg.symdiag_codes) e = cudaMalloc((void **) &pl->d_hcode, (size_t) sd.nd * (size_t) pl->symdiag_stride);
-                if (!e && cfg.symdiag_codes) e = cudaMalloc((void **) &pl->d_codes, sizeof(struct acgb200_codestate));
-                if (e) { *errcode = (int) e; err = ACG_ERR_CUDA; }
+                pl->symdiag_try_codes = cfg.symdiag_codes;
             }
         }
         acgb200_sliceplan_free(&sp);
@@ -863,10 +871,31 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
         if (err) return err;
     }
     pv->plan.max_ctas_per_sm = cfg.spmv_max_ctas;
-    if (pv->plan.nslices > 0) {
-        /* slice-major copy of the covered rows' values, made on the device from the CSR values; with mirrored
-         * diagonals also those and the check that every lower entry equals its mirror bit for bit */
-        struct acgb200_spmvplan *pl = &pv->plan;
+    return fill_values(cg, pv, errcode);
+}
+
+/* Everything of the plan that depends on the matrix values rather than the pattern, made on the device from the
+ * CSR values cg->d_a: the slice-major copy of the covered rows' values; with mirrored diagonals also those, the
+ * check that every lower entry equals its mirror bit for bit and their codes; then the slice kernel's batch and
+ * the grids, which depend on whether the diagonals and their codes were kept.  Run by acgsolvercuda_init and
+ * again by acgsolvercuda_update_values. */
+static int fill_values(struct acgsolvercuda *cg, struct priv *pv, int *errcode)
+{
+    struct acgb200_spmvplan *pl = &pv->plan;
+    if (pl->nslices > 0) {
+        if (pl->symdiag_nd > 0) {
+            /* room for both layouts -- the fill builds and checks the codes from the fp64 diagonals -- and the
+             * check "failed" until it has run and passed; what the values do not allow is freed below */
+            const size_t ne = (size_t) pl->symdiag_nd * (size_t) pl->symdiag_stride;
+            const int one = 1;
+            if (!pl->d_hval) CU(cudaMalloc((void **) &pl->d_hval, ne * sizeof(double)));
+            CU(cudaMalloc((void **) &pl->d_symdiag_bad, sizeof(int)));
+            CU(cudaMemcpy(pl->d_symdiag_bad, &one, sizeof(int), cudaMemcpyHostToDevice));
+            if (pl->symdiag_try_codes && !pl->d_hcode) CU(cudaMalloc((void **) &pl->d_hcode, ne));
+            if (pl->symdiag_try_codes && !pl->d_codes) CU(cudaMalloc((void **) &pl->d_codes, sizeof(struct acgb200_codestate)));
+            pl->symdiag_colidx = cg->d_colidx;
+            pl->symdiag_codes = 0;
+        }
         KL(acgb200_slices_fill(pl, cg->d_rowptr, cg->d_a, pv->stream));
         CU(cudaStreamSynchronize(pv->stream));
         pl->symdiag_colidx = NULL;
@@ -898,10 +927,79 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
             }
         }
         /* batches that divide the row: |O| for the mirrored diagonals, else the most frequent row length */
-        const int d = pl->symdiag_nd > 0 ? pl->symdiag_no : slice_domlen;
-        pl->slice_ub = cfg.slice_ub > 0 ? cfg.slice_ub : (d % 9 == 0 ? 9 : d % 7 == 0 ? 7 : d % 8 == 0 ? 8 : d % 5 == 0 ? 5 : 8);
+        const int d = pl->symdiag_nd > 0 ? pl->symdiag_no : pl->slice_domlen;
+        pl->slice_ub = pl->slice_ub_opt > 0 ? pl->slice_ub_opt
+                                            : (d % 9 == 0 ? 9 : d % 7 == 0 ? 7 : d % 8 == 0 ? 8 : d % 5 == 0 ? 5 : 8);
     }
-    KL(acgb200_spmv_configure(&pv->plan));
+    KL(acgb200_spmv_configure(pl));
+    return ACG_SUCCESS;
+}
+
+/* ACG_SUCCESS if the uploaded matrix ex has the solver's structure (row pointers and columns of both blocks),
+ * ACG_ERR_INVALID_VALUE if it differs.  Compared on the device: only the first differing index comes back. */
+static int same_pattern(const struct acgsolvercuda *cg, const struct priv *pv, const struct acgb200_expanded *ex,
+                        int *errcode)
+{
+    if (ex->fnnz != pv->fnnz || ex->onnz != pv->onnz) return ACG_ERR_INVALID_VALUE;
+    const int64_t nrp = (int64_t) pv->nowned + pv->nghost + 1, norp = (int64_t) pv->nborder + pv->nghost + 1;
+    unsigned long long *d_first = NULL, first = 0;
+    CU(cudaMalloc((void **) &d_first, sizeof(*d_first)));
+    int e = (int) cudaMemsetAsync(d_first, 0xFF, sizeof(*d_first), pv->stream);
+    if (!e) e = acgb200_first_diff(nrp, cg->d_rowptr, ex->d_rowptr, d_first, pv->stream);
+    if (!e) e = acgb200_first_diff(pv->fnnz, cg->d_colidx, ex->d_colidx, d_first, pv->stream);
+    if (!e) e = acgb200_first_diff(norp, cg->d_orowptr, ex->d_orowptr, d_first, pv->stream);
+    if (!e) e = acgb200_first_diff(pv->onnz, cg->d_ocolidx, ex->d_ocolidx, d_first, pv->stream);
+    if (!e) e = (int) cudaMemcpyAsync(&first, d_first, sizeof(first), cudaMemcpyDeviceToHost, pv->stream);
+    if (!e) e = (int) cudaStreamSynchronize(pv->stream);
+    cudaFree(d_first);
+    if (e) { *errcode = e; return ACG_ERR_CUDA; }
+    return first == ~0ULL ? ACG_SUCCESS : ACG_ERR_INVALID_VALUE;
+}
+
+/* ext.h: new values on the solver's pattern */
+int acgsolvercuda_update_values(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, int *errcode)
+{
+    int errcode_ = 0;
+    if (!errcode) errcode = &errcode_;
+    struct priv *pv = cg ? priv_of(cg) : NULL;
+    if (!pv || !A || !matrix_usable(A)) return ACG_ERR_INVALID_VALUE;
+    if (!acgb200_first_diff) return ACG_ERR_NOT_SUPPORTED;     /* the comparison kernel is linked in */
+    if (A->nrows != pv->nrows || A->nownedrows != pv->nowned || A->ninnerrows != pv->ninner
+        || A->nborderrows != pv->nborder || A->nghostrows != pv->nghost || A->borderrowoffset != pv->borderoff
+        || (A->frowptr && (A->fnpnzs != pv->fnnz || A->onpnzs != pv->onnz)))
+        return ACG_ERR_INVALID_VALUE;
+
+    /* the new arrays go to temporaries; the solver's own change only once their structure has been found equal */
+    struct acgb200_expanded ex;
+    OK(upload_matrix(A, &ex, pv->stream, errcode));
+    int err = same_pattern(cg, pv, &ex, errcode);
+    if (!err) {
+        /* in place: every pointer a kernel argument or a captured graph holds stays valid */
+        cudaError_t e = cudaMemcpyAsync(cg->d_a, ex.d_a, (size_t) pv->fnnz * sizeof(double), cudaMemcpyDeviceToDevice,
+                                        pv->stream);
+        if (!e) e = cudaMemcpyAsync(cg->d_oa, ex.d_oa, (size_t) pv->onnz * sizeof(double), cudaMemcpyDeviceToDevice,
+                                    pv->stream);
+        if (!e) e = cudaStreamSynchronize(pv->stream);
+        if (e) { *errcode = (int) e; err = ACG_ERR_CUDA; }
+    }
+    acgb200_expanded_free(&ex);
+    if (err) return err;
+
+    /* what was derived from the old values: the captured loops (their Chebyshev coefficients and the fused
+     * iteration's grid among them), Chebyshev's D^-1, and the fp32 product's row chunks, which leave out the
+     * mirrored diagonals' rows only while the plan keeps them */
+    for (int i = 0; i < NKINDS; i++) {
+        if (pv->graph[i]) cudaGraphExecDestroy(pv->graph[i]);
+        pv->graph[i] = NULL; pv->graph_sig[i] = 0;
+    }
+    pv->cheb_graph_ab[0] = pv->cheb_graph_ab[1] = 0.0;
+    pv->cheb_baddiag = -1;
+    const int had_symdiag = pv->plan.symdiag_nd > 0;
+    OK(fill_values(cg, pv, errcode));
+    if (had_symdiag && pv->plan.symdiag_nd == 0 && pv->have_franges) {
+        cudaFree(pv->d_franges);
+        pv->d_franges = NULL; pv->nfranges = 0; pv->have_franges = 0;
+    }
     return ACG_SUCCESS;
 }
 

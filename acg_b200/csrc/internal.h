@@ -75,6 +75,8 @@ struct acgb200_spmvplan {
     int *d_spatoff;                  /* [slice_npat * slice_lpad] offsets col - row, zero beyond a pattern's length */
     unsigned short *d_spatid;        /* [nrows] pattern id per row (valid for covered rows) */
     int slice_ub, slice_threads, slice_grid, slice_smem, slice_max_ctas;
+    int slice_ub_opt;                /* option "slice_ub" at init (0: slice_ub follows the row length, see slice_domlen) */
+    int slice_domlen;                /* most frequent row length among covered rows (slice_ub without mirrored diagonals) */
     int64_t slice_exc, slice_excnnz; /* exception rows inside slices (columns from the CSR index array) and their nonzeros */
     /* mirrored diagonals (slices.c, acgb200_symdiag_plan): the slice-covered rows of a symmetric matrix read
      * their values from symdiag_nd stored upper diagonals, every lower entry from its mirror row
@@ -93,6 +95,7 @@ struct acgb200_spmvplan {
      * the same layout (d_hcode[voff + i] in place of d_hval[voff + i]) indexes a table of those doubles,
      * sorted by bit pattern.  Built and checked by acgb200_slices_fill when d_hcode and d_codes are set. */
     int symdiag_codes;               /* table entries; 0: the fp64 diagonals */
+    int symdiag_try_codes;           /* option "symdiag_codes" at init: build the coded layout whenever the values allow */
     uint8_t *d_hcode;                /* [symdiag_nd * symdiag_stride] */
     struct acgb200_codestate *d_codes;   /* the table and the state of building it */
     int pcg_grid;                    /* grid of the fused pipelined-CG kernel (acgb200_pcg_fused_launch); 0: none */
@@ -676,6 +679,11 @@ int acgb200_dot(int n, const double *x, const double *y, double *acc, cudaStream
 int acgb200_dot2(int n, const double *r, const double *w, double *acc2, cudaStream_t stream); /* acc2[0]+=r.r, acc2[1]+=w.r */
 int acgb200_gather(int n, double *dst, const double *src, const int *idx, cudaStream_t stream);  /* dst[i]=src[idx[i]] */
 int acgb200_scatter(int n, const double *src, double *dst, const int *idx, cudaStream_t stream); /* dst[idx[i]]=src[i] */
+/* *first = min(*first, the smallest k < n with a[k] != b[k]): set *first to all ones before the first call, and
+ * it still holds all ones afterwards exactly when the arrays agree.  Weak in the host code like the launchers
+ * above: a host-logic test build without it refuses acgsolvercuda_update_values. */
+ACGB200_MULTI_LAUNCHER int acgb200_first_diff(int64_t n, const int *a, const int *b, unsigned long long *first,
+                                              cudaStream_t stream);
 int acgb200_num_sms(void);
 void acgb200_blas1_set_ctas_per_sm(int v);
 void acgb200_set_pdl(int v);

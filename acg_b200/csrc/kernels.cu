@@ -3773,6 +3773,26 @@ extern "C" int acgb200_scatter(int n, const double *src, double *dst, const int 
     return (int) cudaGetLastError();
 }
 
+/* *first = min(*first, the smallest k < n with a[k] != b[k]); a thread stops at its first difference, as every
+ * later index of its stride is larger */
+__global__ void first_diff_kernel(long long n, const int *__restrict__ a, const int *__restrict__ b,
+                                  unsigned long long *__restrict__ first)
+{
+    const long long stride = (long long) gridDim.x * blockDim.x;
+    for (long long k = (long long) blockIdx.x * blockDim.x + threadIdx.x; k < n; k += stride)
+        if (a[k] != b[k]) { atomicMin(first, (unsigned long long) k); return; }
+}
+
+extern "C" int acgb200_first_diff(int64_t n, const int *a, const int *b, unsigned long long *first, cudaStream_t stream)
+{
+    if (n <= 0) return 0;
+    long long grid = (n + 255) / 256;
+    const long long cap = (long long) acgb200_num_sms() * 8;
+    if (grid > cap) grid = cap;
+    first_diff_kernel<<<(int) grid, 256, 0, stream>>>(n, a, b, first);
+    return (int) cudaGetLastError();
+}
+
 /* ------------------------------------------------------------------------ */
 /* BLAS-1 building blocks of acg/cg-kernels-cuda.h:45-97 (public, unused by   */
 /* this library's own loops)                                                  */

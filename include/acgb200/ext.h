@@ -32,6 +32,30 @@ extern "C" {
  * same values at first use. */
 ACG_API int acgb200_set_option(const char *key, int value);
 
+/* Replace the values of the matrix an initialised solver holds, keeping everything that depends only on the
+ * pattern: the tile, slice, mirrored-diagonal and merge plans, row chunks, the halo and peer-memory windows and
+ * the multi-vector blocks.  For a sequence of matrices on one pattern (Newton steps, implicit time steps with
+ * new coefficients, parameter sweeps), at a fraction of acgsolvercuda_free + acgsolvercuda_init.
+ *
+ * A is the matrix the solver was built on or another with the same partition and pattern.  Its values are
+ * taken as acgsolvercuda_init takes them: from its full storage if it has one (frowptr set), else from the
+ * packed triangle, mirrored on the device; either source may be used whichever init used.  After success every
+ * product and solve gives what a solver freshly built on A gives under the options in force at the solver's
+ * acgsolvercuda_init, with one exception: if A's full storage is not exactly symmetric, a solver holding
+ * mirrored diagonals falls back to the slice kernel reading both triangles, as init would, but a later refresh
+ * never re-creates mirrored diagonals that init or an earlier refresh dropped.  Whether the diagonals are stored
+ * as one-byte codes or as doubles follows the new values, as at init.  Cached CUDA graphs are captured again
+ * at the next solve.
+ *
+ * ACG_ERR_INVALID_VALUE, with the solver left exactly as it was: cg is not a live solver; A has neither full
+ * storage nor a packed triangle; the row counts (nrows, nownedrows, ninnerrows, nborderrows, nghostrows,
+ * borderrowoffset) or the entry counts differ from init's; or a row pointer or column of either block differs
+ * (compared on the device).  ACG_ERR_NOT_SUPPORTED, also before any change: a build without the comparison
+ * kernel (host-logic test builds).  A CUDA error after the comparison gives ACG_ERR_CUDA (the third-party code in
+ * *errcode, which may be NULL); the solver is then only fit for acgsolvercuda_free.  Local to a rank, with no
+ * collective: every rank of a partitioned solver refreshes before its next collective solve. */
+ACG_API int acgsolvercuda_update_values(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, int *errcode);
+
 /* y = A*x through the solver's device matrix: the standalone form of the
  * kernel that replaces cusparseSpMV (acg/cgcuda.c:858).  x, y are HOST arrays
  * of nownedrows doubles (unpartitioned matrices only).  If nrep > 0 the kernel
