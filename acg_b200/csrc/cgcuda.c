@@ -171,7 +171,7 @@ struct priv {
     struct acgb200_spmvplan plan;
     struct acgb200_devstate *d_st;
     struct acgb200_ctrl *h_ctrl;        /* pinned, 2 poll slots */
-    struct acgb200_devstate *h_st;      /* pinned scratch for state upload / readback */
+    void *h_st;                         /* pinned staging of every struct of device scalars (scalars_push / _pull) */
     int nrows, nowned, ninner, nborder, nghost, borderoff, nvec;
     int64_t fnnz, onnz;
     int device_expanded;                /* the full storage was built on the device (the host matrix has none) */
@@ -201,21 +201,21 @@ struct priv {
     int last_group;                     /* the group of the last fused solve */
     int commsize;                       /* ranks of the communicator given to acgsolvercuda_init */
     /* several right-hand sides (acgsolvercuda_solve_multi), made at the first multi-vector call */
-    struct acgb200_mstate *d_ms, *h_ms; /* per-column scalars on the device / pinned staging */
+    struct acgb200_mstate *d_ms;        /* per-column scalars */
     double *d_mx, *d_mb, *d_mr, *d_mp, *d_mt;   /* block vectors X, B, R, P, T: nowned x mk, interleaved */
     int mk;                             /* their width */
     int *d_ranges;                      /* [2 * nranges] row chunks outside the pattern slices */
     int nranges, ranges_lanes, have_ranges;
     /* shifted systems (acgsolvercuda_solve_shifted): per-shift scalars; the vectors are the blocks above */
-    struct acgb200_sstate *d_ss, *h_ss;
+    struct acgb200_sstate *d_ss;
     /* MINRES (acgsolvercuda_solve_minres), made at the first such solve: its scalars and the two w buffers
      * (v lives in d_r / d_p, t and u in d_t) */
-    struct acgb200_nstate *d_ns, *h_ns;
+    struct acgb200_nstate *d_ns;
     double *d_nw[2];
     /* mixed precision (acgsolvercuda_solve_mixed), made at the first such solve: its scalars, the float
      * vectors r, p, t, y (one allocation; the fp64 residual lives in d_r) and the row chunks of its product
      * outside the mirrored diagonals */
-    struct acgb200_xstate *d_xs, *h_xs;
+    struct acgb200_xstate *d_xs;
     float *d_f32;
     int *d_franges;
     int nfranges, have_franges;
@@ -223,7 +223,7 @@ struct priv {
     /* Chebyshev-preconditioned CG (acgsolvercuda_solve_chebyshev), made at the first such solve: its scalars
      * and five vectors D^-1, z, res, d_0, d_1 (one allocation); baddiag: the diagonal entries that are <= 0 or
      * non-finite (-1: not counted yet); cheb_graph_ab: the interval whose coefficients the cached graph holds */
-    struct acgb200_cstate *d_cs, *h_cs;
+    struct acgb200_cstate *d_cs;
     double *d_cvec;
     int cheb_baddiag;
     double cheb_graph_ab[2];
@@ -283,6 +283,25 @@ static double wall(void)
 #define KL(call) do { int e_ = (call); if (e_) { if (errcode) *errcode = e_; return ACG_ERR_CUDA; } } while (0)
 #define OK(call) do { int e_ = (call); if (e_) return e_; } while (0)
 
+/* the size of h_st: the largest struct of device scalars */
+static size_t staging_bytes(void)
+{
+    const size_t sizes[] = { sizeof(struct acgb200_devstate), sizeof(struct acgb200_mstate), sizeof(struct acgb200_sstate),
+                             sizeof(struct acgb200_nstate), sizeof(struct acgb200_xstate), sizeof(struct acgb200_cstate) };
+    size_t m = 0;
+    for (size_t i = 0; i < sizeof(sizes) / sizeof(sizes[0]); i++) if (sizes[i] > m) m = sizes[i];
+    return m;
+}
+
+/* a solver's struct of device scalars, made (zeroed) at its first use */
+static int dev_scalars_once(struct priv *pv, void **d, size_t bytes, int *errcode)
+{
+    if (*d) return ACG_SUCCESS;
+    CU(cudaMalloc(d, bytes));
+    CU(cudaMemsetAsync(*d, 0, bytes, pv->stream));
+    return ACG_SUCCESS;
+}
+
 /* ------------------------------------------------------------------------ */
 /* free / init                                                               */
 /* ------------------------------------------------------------------------ */
@@ -329,11 +348,10 @@ void acgsolvercuda_free(struct acgsolvercuda *cg)
         if (pv->redstream) cudaStreamDestroy(pv->redstream);
         if (pv->ev_red) cudaEventDestroy(pv->ev_red);
         cudaFree(pv->d_b); cudaFree(pv->d_x); cudaFree(pv->d_w2); cudaFree(pv->d_rring);
-        cudaFree(pv->d_ms); cudaFreeHost(pv->h_ms); cudaFree(pv->d_ranges);
-        cudaFree(pv->d_ss); cudaFreeHost(pv->h_ss);
-        cudaFree(pv->d_ns); cudaFreeHost(pv->h_ns); cudaFree(pv->d_nw[0]); cudaFree(pv->d_nw[1]);
-        cudaFree(pv->d_xs); cudaFreeHost(pv->h_xs); cudaFree(pv->d_f32); cudaFree(pv->d_franges);
-        cudaFree(pv->d_cs); cudaFreeHost(pv->h_cs); cudaFree(pv->d_cvec);
+        cudaFree(pv->d_ms); cudaFree(pv->d_ranges); cudaFree(pv->d_ss);
+        cudaFree(pv->d_ns); cudaFree(pv->d_nw[0]); cudaFree(pv->d_nw[1]);
+        cudaFree(pv->d_xs); cudaFree(pv->d_f32); cudaFree(pv->d_franges);
+        cudaFree(pv->d_cs); cudaFree(pv->d_cvec);
         cudaFree(pv->d_mx); cudaFree(pv->d_mb); cudaFree(pv->d_mr); cudaFree(pv->d_mp); cudaFree(pv->d_mt);
         if (pv->ev_ready) cudaEventDestroy(pv->ev_ready);
         if (pv->ev_halo) cudaEventDestroy(pv->ev_halo);
@@ -683,6 +701,7 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
     struct priv *pv = calloc(1, sizeof(*pv));
     if (!pv) return ACG_ERR_ERRNO;
     pv->key = cg;
+    pv->cheb_baddiag = -1;              /* D^-1 is made at the first Chebyshev solve */
     priv_add(pv);
 
     /* host-side work vectors, as the reference keeps them (acg/cgcuda.c:145-153) */
@@ -760,7 +779,7 @@ static int init_impl(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, 
     CU(cudaMalloc((void **) &pv->d_st, sizeof(*pv->d_st)));
     CU(cudaMemset(pv->d_st, 0, sizeof(*pv->d_st)));
     CU(cudaMallocHost((void **) &pv->h_ctrl, 2 * sizeof(*pv->h_ctrl)));
-    CU(cudaMallocHost((void **) &pv->h_st, sizeof(*pv->h_st)));
+    CU(cudaMallocHost(&pv->h_st, staging_bytes()));
 
     /* device vectors: owned + ghost entries, padded to an even count */
     const size_t vbytes = ((size_t) pv->nvec + 2) * sizeof(double);
@@ -1014,6 +1033,9 @@ struct solvectx {
     int multi, tag;
     int *errcode;
     double *d_b, *d_x;
+    struct acgvector *x;      /* where solve_finish brings x back: the caller's vector, or */
+    double *X;                /* the nrhs columns of the X block (host, row-major) */
+    int nrhs;
     int launches;
     int capturing;            /* inside cudaStreamBeginCapture: no profiling marks */
     int p2p;                  /* loop exchanges go through peer memory */
@@ -1107,13 +1129,6 @@ static int window_close(struct solvectx *c)
         cg->taxpy += 1e-3 * pv->last_blas_ms;
     }
     return ACG_SUCCESS;
-}
-
-/* the return-code rule of acg/cgcuda.c:1099-1107: a solve that did not converge fails unless both
- * tolerances are off */
-static int not_converged(int converged, double atol, double rtol_scaled)
-{
-    return !converged && !(atol == 0 && rtol_scaled == 0);
 }
 
 /* offdiag_kernel's share of the epilogue of `mode` (o->acc set): add the border x ghost block to
@@ -1228,18 +1243,31 @@ static int allreduce(struct solvectx *c, const double *src, double *dst, int cou
 }
 
 /* the communicator of the one-GPU entry points */
-static struct acgcomm null_comm(void)
-{
-    struct acgcomm null;
-    memset(&null, 0, sizeof(null));
-    null.type = acgcomm_null;
-    return null;
-}
+static struct acgcomm one_gpu_comm = { .type = acgcomm_null };
 
-/* one GPU, whole matrix: what the multi-vector, shifted, MINRES and mixed-precision paths support */
+/* one GPU, whole matrix: what the multi-vector, shifted, MINRES, mixed-precision and Chebyshev paths support */
 static int one_gpu(const struct priv *pv, const struct acgsymcsrmatrix *A)
 {
     return pv->nghost == 0 && pv->commsize == 1 && !(A && A->nghostrows > 0);
+}
+
+/* The refusals of a one-GPU entry point, in this order: an unknown solver or a missing argument
+ * (ACG_ERR_INVALID_VALUE), missing kernels or a partitioned matrix (ACG_ERR_NOT_SUPPORTED), then arguments out of
+ * range (ACG_ERR_INVALID_VALUE).  A refused call changes nothing. */
+static int one_gpu_entry(struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A, int args_given, int have_kernels,
+                         int args_valid, struct priv **pv)
+{
+    cfg_load();
+    *pv = priv_of(cg);
+    if (!*pv || !args_given) return ACG_ERR_INVALID_VALUE;
+    if (!have_kernels || !one_gpu(*pv, A)) return ACG_ERR_NOT_SUPPORTED;
+    return args_valid ? ACG_SUCCESS : ACG_ERR_INVALID_VALUE;
+}
+
+static void ctx_init(struct solvectx *c, struct acgsolvercuda *cg, struct priv *pv, int *errcode)
+{
+    memset(c, 0, sizeof(*c));
+    c->cg = cg; c->pv = pv; c->errcode = errcode;
 }
 
 /* global sum of a device-side reduction result, brought to the host */
@@ -1252,25 +1280,68 @@ static int reduce_to_host(struct solvectx *c, double *loc, double *glob, int cou
     return ACG_SUCCESS;
 }
 
-/* x0 from the caller's vector to the device; the time goes to last_h2d_ms */
-static int upload_x0(struct solvectx *c, const struct acgvector *x)
+/* n x nrhs row-major host array <-> n x k interleaved device block (padding columns zero); with nrhs = k = 1,
+ * n entries of a vector */
+static int upload_block_vec(struct priv *pv, double *dst, const double *src, size_t n, int nrhs, int k, int *errcode)
 {
-    struct priv *pv = c->pv;
-    int *errcode = c->errcode;
-    const double tb = wall();
-    /* a caller may hand over a longer vector than this part's owned + ghost entries: only those are used */
-    const size_t nx = (size_t) (x->num_nonzeros < pv->nvec ? x->num_nonzeros : pv->nvec);
-    CU(cudaMemcpyAsync(c->d_x, x->x, nx * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
-    CU(cudaStreamSynchronize(pv->stream));
-    pv->last_h2d_ms += 1e3 * (wall() - tb);
+    if (nrhs == k) {
+        CU(cudaMemcpyAsync(dst, src, n * (size_t) k * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
+        CU(cudaStreamSynchronize(pv->stream));
+        return ACG_SUCCESS;
+    }
+    double *tmp = calloc(n * (size_t) k + 1, sizeof(double));
+    if (!tmp) return ACG_ERR_ERRNO;
+    for (size_t i = 0; i < n; i++) memcpy(tmp + i * (size_t) k, src + i * (size_t) nrhs, (size_t) nrhs * sizeof(double));
+    cudaError_t e = cudaMemcpyAsync(dst, tmp, n * (size_t) k * sizeof(double), cudaMemcpyHostToDevice, pv->stream);
+    if (!e) e = cudaStreamSynchronize(pv->stream);
+    free(tmp);
+    CU(e);
     return ACG_SUCCESS;
 }
 
+static int download_block_vec(struct priv *pv, double *dst, const double *src, size_t n, int nrhs, int k, int *errcode)
+{
+    if (nrhs == k) {
+        CU(cudaMemcpyAsync(dst, src, n * (size_t) k * sizeof(double), cudaMemcpyDeviceToHost, pv->stream));
+        CU(cudaStreamSynchronize(pv->stream));
+        return ACG_SUCCESS;
+    }
+    double *tmp = malloc((n * (size_t) k + 1) * sizeof(double));
+    if (!tmp) return ACG_ERR_ERRNO;
+    cudaError_t e = cudaMemcpyAsync(tmp, src, n * (size_t) k * sizeof(double), cudaMemcpyDeviceToHost, pv->stream);
+    if (!e) e = cudaStreamSynchronize(pv->stream);
+    if (!e) for (size_t i = 0; i < n; i++) memcpy(dst + i * (size_t) nrhs, tmp + i * (size_t) k, (size_t) nrhs * sizeof(double));
+    free(tmp);
+    CU(e);
+    return ACG_SUCCESS;
+}
+
+/* an upload before the solve window; its host time goes to last_h2d_ms */
+static int upload(struct solvectx *c, double *dst, const double *src, size_t n, int nrhs, int k)
+{
+    const double tb = wall();
+    OK(upload_block_vec(c->pv, dst, src, n, nrhs, k, c->errcode));
+    c->pv->last_h2d_ms += 1e3 * (wall() - tb);
+    return ACG_SUCCESS;
+}
+
+/* a caller may hand over a longer vector than this part's owned + ghost entries: only those are used */
+static size_t vec_entries(const struct priv *pv, const struct acgvector *v)
+{
+    return (size_t) (v->num_nonzeros < pv->nvec ? v->num_nonzeros : pv->nvec);
+}
+
+/* x0 from the caller's vector to the device */
+static int upload_x0(struct solvectx *c, const struct acgvector *x)
+{
+    return upload(c, c->d_x, x->x, vec_entries(c->pv, x), 1, 1);
+}
+
+/* The context of a solve of vectors b, x of `kind`: b and x0 on the device */
 static int solve_begin(struct solvectx *c, struct acgsolvercuda *cg, const struct acgsymcsrmatrix *A,
                        const struct acgvector *b, struct acgvector *x, double diffatol, double diffrtol,
-                       struct acgcomm *comm, int tag, int *errcode)
+                       struct acgcomm *comm, int tag, enum solve_kind kind, int *errcode)
 {
-    memset(c, 0, sizeof(*c));
     if (b->size < A->nrows || x->size < A->nrows || cg->r.size < A->nrows ||
         cg->p.size < A->nrows || cg->t.size < A->nrows) return ACG_ERR_INDEX_OUT_OF_BOUNDS;
     if (diffatol > 0 || diffrtol > 0) return ACG_ERR_NOT_SUPPORTED;     /* acg/cgcuda.c:424 */
@@ -1279,13 +1350,13 @@ static int solve_begin(struct solvectx *c, struct acgsolvercuda *cg, const struc
     if (b->num_nonzeros < pv->nowned || x->num_nonzeros < pv->nvec) return ACG_ERR_VECTOR_INCOMPATIBLE_SIZE;
     int commsize = 1;
     OK(acgcomm_size(comm, &commsize));
-    c->cg = cg; c->pv = pv; c->comm = comm; c->multi = commsize > 1; c->tag = tag; c->errcode = errcode;
+    ctx_init(c, cg, pv, errcode);
+    c->comm = comm; c->multi = commsize > 1; c->tag = tag; c->kind = kind; c->x = x;
     if (c->multi && comm->type != acgcomm_nccl)
         return comm->type == acgcomm_mpi ? ACG_ERR_MPI_NOT_SUPPORTED : ACG_ERR_NVSHMEM_NOT_SUPPORTED;
     /* b and x0 to the device (acg/cgcuda.c:484-493).  The reference allocates and
      * frees the two device vectors in every solve; here they are kept with the
      * solver (their addresses are baked into the replayed CUDA graphs). */
-    const double tb = wall();
     const size_t vbytes = ((size_t) pv->nvec + 2) * sizeof(double);
     if (!pv->d_b) {
         CU(cudaMalloc((void **) &pv->d_b, vbytes));
@@ -1294,43 +1365,65 @@ static int solve_begin(struct solvectx *c, struct acgsolvercuda *cg, const struc
         CU(cudaMemsetAsync(pv->d_x, 0, vbytes, pv->stream));
     }
     c->d_b = pv->d_b; c->d_x = pv->d_x;
-    const size_t nb = (size_t) (b->num_nonzeros < pv->nvec ? b->num_nonzeros : pv->nvec);
-    CU(cudaMemcpyAsync(c->d_b, b->x, nb * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
-    pv->last_h2d_ms = 1e3 * (wall() - tb);
+    pv->last_h2d_ms = 0;
+    OK(upload(c, c->d_b, b->x, vec_entries(pv, b), 1, 1));
     return upload_x0(c, x);
 }
 
-static int solve_end(struct solvectx *c, struct acgvector *x, int status)
+/* The context of a solve of `kind` on the K-wide blocks; the caller uploads into them, and X gets the nrhs columns
+ * of the X block back */
+static void block_begin(struct solvectx *c, struct acgsolvercuda *cg, struct priv *pv, enum solve_kind kind, int K,
+                        double *X, int nrhs, int *errcode)
 {
+    ctx_init(c, cg, pv, errcode);
+    c->kind = kind; c->mk = K; c->X = X; c->nrhs = nrhs;
+    c->d_b = pv->d_mb; c->d_x = pv->d_mx;
+    pv->last_h2d_ms = 0;
+}
+
+/* the return-code rule of acg/cgcuda.c:1099-1107: a solve that did not converge fails unless both
+ * tolerances are off */
+static int convergence_status(int converged, double atol, double rtol_scaled)
+{
+    return !converged && !(atol == 0 && rtol_scaled == 0) ? ACG_ERR_NOT_CONVERGED : ACG_SUCCESS;
+}
+
+/* The end of every solve, after its counters are charged: ntotaliterations, the window closed, x (or the columns
+ * of X) back on the host, the time of that in last_d2h_ms, and `status` unless the device reports an error */
+static int solve_finish(struct solvectx *c, int status)
+{
+    struct priv *pv = c->pv;
     int *errcode = c->errcode;
+    c->cg->ntotaliterations += c->cg->niterations;
+    OK(window_close(c));
     const double te = wall();
-    const size_t nx = (size_t) (x->num_nonzeros < c->pv->nvec ? x->num_nonzeros : c->pv->nvec);
-    CU(cudaMemcpyAsync(x->x, c->d_x, nx * sizeof(double), cudaMemcpyDeviceToHost, c->pv->stream));
-    CU(cudaStreamSynchronize(c->pv->stream));
-    c->pv->last_d2h_ms = 1e3 * (wall() - te);
+    if (c->X) OK(download_block_vec(pv, c->X, c->d_x, (size_t) pv->nowned, c->nrhs, c->mk, errcode));
+    else OK(download_block_vec(pv, c->x->x, c->d_x, vec_entries(pv, c->x), 1, 1, errcode));
+    pv->last_d2h_ms = 1e3 * (wall() - te);
     CU(cudaGetLastError());
     return status;
 }
 
-/* one struct of device scalars (d_st, d_ms, d_ss, d_ns, d_xs) from the host through its pinned staging buffer */
-static int scalars_push(struct solvectx *c, void *dev, void *pinned, const void *src, size_t bytes)
+/* one struct of device scalars (d_st, d_ms, d_ss, d_ns, d_xs, d_cs) from the host through the pinned staging
+ * buffer h_st; both transfers are synchronous, so one buffer serves every struct */
+static int scalars_push(struct solvectx *c, void *dev, const void *src, size_t bytes)
 {
     int *errcode = c->errcode;
     /* everything queued before must be done with the staging buffer and with
      * the device state it is about to replace */
     CU(cudaStreamSynchronize(c->pv->stream));
-    memcpy(pinned, src, bytes);
-    CU(cudaMemcpyAsync(dev, pinned, bytes, cudaMemcpyHostToDevice, c->pv->stream));
+    memcpy(c->pv->h_st, src, bytes);
+    CU(cudaMemcpyAsync(dev, c->pv->h_st, bytes, cudaMemcpyHostToDevice, c->pv->stream));
     CU(cudaStreamSynchronize(c->pv->stream));
     return ACG_SUCCESS;
 }
 
-static int scalars_pull(struct solvectx *c, const void *dev, void *pinned, void *dst, size_t bytes)
+static int scalars_pull(struct solvectx *c, const void *dev, void *dst, size_t bytes)
 {
     int *errcode = c->errcode;
-    CU(cudaMemcpyAsync(pinned, dev, bytes, cudaMemcpyDeviceToHost, c->pv->stream));
+    CU(cudaMemcpyAsync(c->pv->h_st, dev, bytes, cudaMemcpyDeviceToHost, c->pv->stream));
     CU(cudaStreamSynchronize(c->pv->stream));
-    memcpy(dst, pinned, bytes);
+    memcpy(dst, c->pv->h_st, bytes);
     return ACG_SUCCESS;
 }
 
@@ -1342,6 +1435,65 @@ static double threshold(double atol, double rtol, double r0nrm2)
     if (atol > 0) t = atol;
     if (rtol * r0nrm2 > t) t = rtol * r0nrm2;
     return t;
+}
+
+/* the stopping test at r0 (acg/cgcuda.c:836-842): its threshold, rtol ||r0|| for convergence_status, and whether
+ * r0 meets it */
+static int r0_test(double atol, double rtol, double r0nrm2, double *tol, double *rtol_scaled)
+{
+    *tol = threshold(atol, rtol, r0nrm2);
+    *rtol_scaled = rtol * r0nrm2;
+    return *tol > 0 && r0nrm2 < *tol;
+}
+
+/* (b, b) into *bb and cg->bnrm2 (acg/cgcuda.c:727-739), the scalars zeroed first; `setup` (if given) is issued
+ * between the two */
+static int rhs_norm(struct solvectx *c, int (*setup)(struct solvectx *), double *bb)
+{
+    struct priv *pv = c->pv;
+    int *errcode = c->errcode;
+    struct acgb200_devstate h;
+    memset(&h, 0, sizeof(h));
+    OK(scalars_push(c, pv->d_st, &h, sizeof(h)));
+    if (setup) OK(setup(c));
+    KL(acgb200_dot(pv->nowned, c->d_b, c->d_b, &pv->d_st->tmp_loc[0], pv->stream));
+    OK(reduce_to_host(c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, bb));
+    c->cg->bnrm2 = sqrt(*bb);
+    return ACG_SUCCESS;
+}
+
+/* r = b - A x into d_r with (r, r) folded in (ungated, the scalars zeroed first), (r, r) into *rr: the r0 of
+ * MINRES, mixed-precision and Chebyshev CG, and the fp64 residual of a mixed-precision x */
+static int residual(struct solvectx *c, double *rr)
+{
+    struct priv *pv = c->pv;
+    struct acgb200_devstate h;
+    memset(&h, 0, sizeof(h));
+    OK(scalars_push(c, pv->d_st, &h, sizeof(h)));
+    *rr = 0;
+    OK(apply_A(c, c->d_x, c->d_x, c->cg->d_r, c->d_b, SPMV_R_B_AX, &pv->d_st->tmp_loc[0], 0, 0, 0, -1));
+    return reduce_to_host(c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, rr);
+}
+
+/* The results of a solve of several columns (right-hand sides or shifts) from their squared norms: each column's
+ * stats (if asked), the norms of the solver as those of the whole block, and the status by the rule of
+ * convergence_status per column */
+static int column_results(struct acgsolvercuda *cg, int ncols, const int *nits, const int *conv, const double *bb,
+                          const double *rr0, const double *rr, double atol, const double *rtol_scaled,
+                          struct acgb200_colstats *stats)
+{
+    double sb = 0, sr0 = 0, sr = 0;
+    int status = ACG_SUCCESS;
+    for (int j = 0; j < ncols; j++) {
+        sb += bb[j]; sr0 += rr0[j]; sr += rr[j];
+        if (convergence_status(conv[j], atol, rtol_scaled[j])) status = ACG_ERR_NOT_CONVERGED;
+        if (stats) {
+            stats[j].niterations = nits[j]; stats[j].converged = conv[j];
+            stats[j].bnrm2 = sqrt(bb[j]); stats[j].r0nrm2 = sqrt(rr0[j]); stats[j].rnrm2 = sqrt(rr[j]);
+        }
+    }
+    cg->bnrm2 = sqrt(sb); cg->r0nrm2 = sqrt(sr0); cg->rnrm2 = sqrt(sr);
+    return status;
 }
 
 /* Capture iterations g ... 2g - 1 of `issue` into a graph (g = graph_group).  All
@@ -1500,13 +1652,12 @@ int acgsolvercuda_solvempi(
     if (!errcode) errcode = &errcode_;
     cfg_load();
     struct solvectx c;
-    OK(solve_begin(&c, cg, A, b, x, diffatol, diffrtol, comm, tag, errcode));
+    OK(solve_begin(&c, cg, A, b, x, diffatol, diffrtol, comm, tag, KIND_CLASSIC, errcode));
     struct priv *pv = c.pv;
     struct acgb200_devstate *st = pv->d_st;
     const int n = pv->nowned;
     struct acgb200_devstate h;
 
-    c.kind = KIND_CLASSIC;
     c.p2p = c.multi && pv->p2p.enabled && cfg.p2p;
     /* a rank that is ahead must not store into a peer's window while that peer's kernels of the
      * previous solve are still reading it: order the first post of this solve behind every rank */
@@ -1518,7 +1669,7 @@ int acgsolvercuda_solvempi(
     if (warmup > 0) {
         memset(&h, 0, sizeof(h));
         h.maxits = warmup; h.rr_loc[0] = h.rr[0] = 1.0;
-        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_push(&c, pv->d_st, &h, sizeof(h)));
         double *xsave = c.d_x; c.d_x = cg->d_r;
         if (c.p2p) {
             OK(acgb200_p2p_begin(&pv->p2p, warmup, pv->stream));
@@ -1531,13 +1682,8 @@ int acgsolvercuda_solvempi(
     }
     OK(window_open(&c, maxits, residualatol, residualrtol, diffatol, diffrtol));
 
-    /* ||b|| (acg/cgcuda.c:727-739) */
-    memset(&h, 0, sizeof(h));
-    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
-    double bb = 0, rr0 = 0;
-    KL(acgb200_dot(n, c.d_b, c.d_b, &st->tmp_loc[0], pv->stream));
-    OK(reduce_to_host(&c, &st->tmp_loc[0], &st->tmp[0], 1, &bb));
-    cg->bnrm2 = sqrt(bb);
+    double bb = 0, rr0 = 0, tol = 0, rtol_scaled = 0;
+    OK(rhs_norm(&c, NULL, &bb));
     cg->nnrm2++; cg->nflops += 2 * (int64_t) n; cg->Bnrm2 += 8 * (int64_t) n;
 
     /* r0 = b - A x0 with (r0,r0) folded in (acg/cgcuda.c:761-799,:819-832); p = r0 */
@@ -1546,32 +1692,28 @@ int acgsolvercuda_solvempi(
     OK(reduce_to_host(&c, &st->rr_loc[0], &st->rr[0], 1, &rr0));
     cg->rnrm2 = cg->r0nrm2 = sqrt(rr0);
     cg->ngemv++; cg->ncopy += 2; cg->nnrm2++;
-    const double tol = threshold(residualatol, residualrtol, cg->r0nrm2);
-    const double rtol_scaled = residualrtol * cg->r0nrm2;
-    int converged = tol > 0 && cg->rnrm2 < tol;                    /* acg/cgcuda.c:836-842 */
+    int converged = r0_test(residualatol, residualrtol, cg->r0nrm2, &tol, &rtol_scaled);
 
     if (!converged && maxits > 0) {
         memset(&h, 0, sizeof(h));
         h.maxits = maxits; h.tol = tol;
         h.rr_loc[0] = h.rr[0] = rr0;
-        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_push(&c, pv->d_st, &h, sizeof(h)));
         if (c.p2p) {
             /* p_0 = r_0 goes to the neighbours' windows as exchange number 0 */
             OK(acgb200_p2p_begin(&pv->p2p, maxits, pv->stream));
             OK(post(&c, 0, 0, pvec, -1, NULL, 0, 0, 0, 0));
         }
         OK(iterate(&c, maxits, tol > 0, classic_iteration));
-        OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_pull(&c, pv->d_st, &h, sizeof(h)));
         cg->niterations = h.ctrl[0].iter;
         converged = h.ctrl[0].done;
         const double rr = converged ? h.final_rr
             : (c.multi ? h.rr[cg->niterations & 1] : h.rr_loc[cg->niterations & 1]);
         cg->rnrm2 = sqrt(rr);
-        cg->ntotaliterations += cg->niterations;
     }
-    OK(window_close(&c));
     account_classic(cg, pv, cg->niterations, c.multi);
-    return solve_end(&c, x, not_converged(converged, residualatol, rtol_scaled) ? ACG_ERR_NOT_CONVERGED : ACG_SUCCESS);
+    return solve_finish(&c, convergence_status(converged, residualatol, rtol_scaled));
 }
 
 int acgsolvercuda_solve(
@@ -1579,10 +1721,9 @@ int acgsolvercuda_solve(
     const struct acgvector *b, struct acgvector *x,
     int maxits, double diffatol, double diffrtol, double residualatol, double residualrtol, int warmup)
 {
-    struct acgcomm null = null_comm();
     int errcode = 0;
     return acgsolvercuda_solvempi(cg, A, b, x, maxits, diffatol, diffrtol, residualatol, residualrtol,
-                                  warmup, &null, 0, &errcode, NULL, NULL, 0);
+                                  warmup, &one_gpu_comm, 0, &errcode, NULL, NULL, 0);
 }
 
 /* ------------------------------------------------------------------------ */
@@ -1649,11 +1790,7 @@ static int build_ranges(struct priv *pv, const struct acgsolvercuda *cg, int *er
  * blocks (and the captured multi-vector loop, whose pointers they were) */
 static int ensure_blocks(struct priv *pv, const struct acgsolvercuda *cg, int k, int *errcode)
 {
-    if (!pv->d_ms) {
-        CU(cudaMalloc((void **) &pv->d_ms, sizeof(*pv->d_ms)));
-        CU(cudaMemsetAsync(pv->d_ms, 0, sizeof(*pv->d_ms), pv->stream));
-        CU(cudaMallocHost((void **) &pv->h_ms, sizeof(*pv->h_ms)));
-    }
+    OK(dev_scalars_once(pv, (void **) &pv->d_ms, sizeof(*pv->d_ms), errcode));
     OK(build_ranges(pv, cg, errcode));
     if (pv->mk >= k) return ACG_SUCCESS;
     double **blk[5] = { &pv->d_mx, &pv->d_mb, &pv->d_mr, &pv->d_mp, &pv->d_mt };
@@ -1669,43 +1806,6 @@ static int ensure_blocks(struct priv *pv, const struct acgsolvercuda *cg, int k,
         CU(cudaMemsetAsync(*blk[i], 0, bytes, pv->stream));
     }
     pv->mk = k;
-    return ACG_SUCCESS;
-}
-
-/* n x nrhs row-major host array <-> n x k interleaved device block (padding columns zero) */
-static int upload_block_vec(struct priv *pv, double *dst, const double *src, int nrhs, int k, int *errcode)
-{
-    const size_t n = (size_t) pv->nowned;
-    if (nrhs == k) {
-        CU(cudaMemcpyAsync(dst, src, n * (size_t) k * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
-        CU(cudaStreamSynchronize(pv->stream));
-        return ACG_SUCCESS;
-    }
-    double *tmp = calloc(n * (size_t) k + 1, sizeof(double));
-    if (!tmp) return ACG_ERR_ERRNO;
-    for (size_t i = 0; i < n; i++) memcpy(tmp + i * (size_t) k, src + i * (size_t) nrhs, (size_t) nrhs * sizeof(double));
-    cudaError_t e = cudaMemcpyAsync(dst, tmp, n * (size_t) k * sizeof(double), cudaMemcpyHostToDevice, pv->stream);
-    if (!e) e = cudaStreamSynchronize(pv->stream);
-    free(tmp);
-    CU(e);
-    return ACG_SUCCESS;
-}
-
-static int download_block_vec(struct priv *pv, double *dst, const double *src, int nrhs, int k, int *errcode)
-{
-    const size_t n = (size_t) pv->nowned;
-    if (nrhs == k) {
-        CU(cudaMemcpyAsync(dst, src, n * (size_t) k * sizeof(double), cudaMemcpyDeviceToHost, pv->stream));
-        CU(cudaStreamSynchronize(pv->stream));
-        return ACG_SUCCESS;
-    }
-    double *tmp = malloc((n * (size_t) k + 1) * sizeof(double));
-    if (!tmp) return ACG_ERR_ERRNO;
-    cudaError_t e = cudaMemcpyAsync(tmp, src, n * (size_t) k * sizeof(double), cudaMemcpyDeviceToHost, pv->stream);
-    if (!e) e = cudaStreamSynchronize(pv->stream);
-    if (!e) for (size_t i = 0; i < n; i++) memcpy(dst + i * (size_t) nrhs, tmp + i * (size_t) k, (size_t) nrhs * sizeof(double));
-    free(tmp);
-    CU(e);
     return ACG_SUCCESS;
 }
 
@@ -1762,21 +1862,14 @@ int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acgsymcsrma
                               int warmup, struct acgb200_colstats *stats)
 {
     int errcode_ = 0, *errcode = &errcode_;
-    cfg_load();
-    struct priv *pv = priv_of(cg);
-    if (!pv) return ACG_ERR_INVALID_VALUE;
-    if (!have_multi_kernels() || !one_gpu(pv, A)) return ACG_ERR_NOT_SUPPORTED;
-    if (nrhs < 1 || nrhs > ACGB200_MAXK || !B || !X || maxits < 0) return ACG_ERR_INVALID_VALUE;
+    struct priv *pv;
+    OK(one_gpu_entry(cg, A, 1, have_multi_kernels(), nrhs >= 1 && nrhs <= ACGB200_MAXK && B && X && maxits >= 0, &pv));
     const int K = block_width(nrhs), n = pv->nowned;
     OK(ensure_blocks(pv, cg, K, errcode));
     struct solvectx c;
-    memset(&c, 0, sizeof(c));
-    c.cg = cg; c.pv = pv; c.errcode = errcode; c.mk = K; c.kind = KIND_MULTI;
-    c.d_b = pv->d_mb; c.d_x = pv->d_mx;
-    const double tb = wall();
-    OK(upload_block_vec(pv, pv->d_mb, B, nrhs, K, errcode));
-    OK(upload_block_vec(pv, pv->d_mx, X, nrhs, K, errcode));
-    pv->last_h2d_ms = 1e3 * (wall() - tb);
+    block_begin(&c, cg, pv, KIND_MULTI, K, X, nrhs, errcode);
+    OK(upload(&c, c.d_b, B, (size_t) n, nrhs, K));
+    OK(upload(&c, c.d_x, X, (size_t) n, nrhs, K));
     struct acgb200_devstate h;
     struct acgb200_mstate m;
 
@@ -1785,10 +1878,10 @@ int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acgsymcsrma
     if (warmup > 0) {
         memset(&m, 0, sizeof(m));
         for (int j = 0; j < ACGB200_MAXK; j++) m.rr[0][j] = 1.0;
-        OK(scalars_push(&c, pv->d_ms, pv->h_ms, &m, sizeof(m)));
+        OK(scalars_push(&c, pv->d_ms, &m, sizeof(m)));
         memset(&h, 0, sizeof(h));
         h.maxits = warmup; h.ctrl[0].pad0 = (1 << K) - 1;
-        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_push(&c, pv->d_st, &h, sizeof(h)));
         c.d_x = pv->d_mr;
         for (int i = 0; i < warmup; i++) OK(multi_iteration(&c, i));
         c.d_x = pv->d_mx;
@@ -1799,22 +1892,20 @@ int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acgsymcsrma
 
     /* ||b_j|| ; r0 = B - A X0 with (r0_j,r0_j) folded in ; P = R */
     memset(&h, 0, sizeof(h));
-    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+    OK(scalars_push(&c, pv->d_st, &h, sizeof(h)));
     memset(&m, 0, sizeof(m));
-    OK(scalars_push(&c, pv->d_ms, pv->h_ms, &m, sizeof(m)));
+    OK(scalars_push(&c, pv->d_ms, &m, sizeof(m)));
     KL(acgb200_dot_multi(n, K, pv->d_mb, &pv->d_ms->tmp[0], pv->stream));
     OK(apply_A_multi(&c, pv->d_mx, pv->d_mr, pv->d_mb, SPMV_R_B_AX, &pv->d_ms->rr[0][0], 0));
     CU(cudaMemcpyAsync(pv->d_mp, pv->d_mr, (size_t) n * K * sizeof(double), cudaMemcpyDeviceToDevice, pv->stream));
-    OK(scalars_pull(&c, pv->d_ms, pv->h_ms, &m, sizeof(m)));
+    OK(scalars_pull(&c, pv->d_ms, &m, sizeof(m)));
     c.launches += 1;
     double bb[ACGB200_MAXK], rr0[ACGB200_MAXK], tol[ACGB200_MAXK], rtol_scaled[ACGB200_MAXK];
     unsigned mask = 0;
     int poll = 0;
     for (int j = 0; j < nrhs; j++) {
         bb[j] = m.tmp[j]; rr0[j] = m.rr[0][j];
-        tol[j] = threshold(residualatol, residualrtol, sqrt(rr0[j]));
-        rtol_scaled[j] = residualrtol * sqrt(rr0[j]);
-        if (!(tol[j] > 0 && sqrt(rr0[j]) < tol[j])) mask |= 1u << j;       /* acg/cgcuda.c:836-842 per column */
+        if (!r0_test(residualatol, residualrtol, sqrt(rr0[j]), &tol[j], &rtol_scaled[j])) mask |= 1u << j;
         if (tol[j] > 0) poll = 1;
     }
     int nits[ACGB200_MAXK], conv[ACGB200_MAXK];
@@ -1823,37 +1914,20 @@ int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acgsymcsrma
     if (maxits > 0 && mask) {
         memset(&m, 0, sizeof(m));
         for (int j = 0; j < nrhs; j++) { m.tol[j] = tol[j]; m.rr[0][j] = rr0[j]; m.final_rr[j] = rr0[j]; }
-        OK(scalars_push(&c, pv->d_ms, pv->h_ms, &m, sizeof(m)));
+        OK(scalars_push(&c, pv->d_ms, &m, sizeof(m)));
         memset(&h, 0, sizeof(h));
         h.maxits = maxits; h.ctrl[0].pad0 = (int) mask;
-        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_push(&c, pv->d_st, &h, sizeof(h)));
         OK(iterate(&c, maxits, poll, multi_iteration));
-        OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
-        OK(scalars_pull(&c, pv->d_ms, pv->h_ms, &m, sizeof(m)));
+        OK(scalars_pull(&c, pv->d_st, &h, sizeof(h)));
+        OK(scalars_pull(&c, pv->d_ms, &m, sizeof(m)));
         cg->niterations = h.ctrl[0].iter;
         for (int j = 0; j < nrhs; j++)
             if (mask >> j & 1u) { nits[j] = m.nits[j]; conv[j] = m.conv[j]; rr[j] = m.final_rr[j]; }
     }
-    cg->ntotaliterations += cg->niterations;
-    OK(window_close(&c));
     account_multi(cg, pv, cg->niterations, K);
     cg->ngemv++; cg->ncopy += 1; cg->nnrm2 += 2 * nrhs;
-    double sb = 0, sr0 = 0, sr = 0;
-    int status = ACG_SUCCESS;
-    for (int j = 0; j < nrhs; j++) {
-        sb += bb[j]; sr0 += rr0[j]; sr += rr[j];
-        if (not_converged(conv[j], residualatol, rtol_scaled[j])) status = ACG_ERR_NOT_CONVERGED;      /* per column */
-        if (stats) {
-            stats[j].niterations = nits[j]; stats[j].converged = conv[j];
-            stats[j].bnrm2 = sqrt(bb[j]); stats[j].r0nrm2 = sqrt(rr0[j]); stats[j].rnrm2 = sqrt(rr[j]);
-        }
-    }
-    cg->bnrm2 = sqrt(sb); cg->r0nrm2 = sqrt(sr0); cg->rnrm2 = sqrt(sr);
-    const double te = wall();
-    OK(download_block_vec(pv, X, pv->d_mx, nrhs, K, errcode));
-    pv->last_d2h_ms = 1e3 * (wall() - te);
-    CU(cudaGetLastError());
-    return status;
+    return solve_finish(&c, column_results(cg, nrhs, nits, conv, bb, rr0, rr, residualatol, rtol_scaled, stats));
 }
 
 /* ------------------------------------------------------------------------ */
@@ -1864,6 +1938,22 @@ int acgsolvercuda_solve_multi(struct acgsolvercuda *cg, const struct acgsymcsrma
 static int have_shift_kernels(void)
 {
     return have_multi_kernels() && acgb200_shift_setup && acgb200_cg_shift_update;
+}
+
+/* 1 ... ACGB200_MAXK shifts, each finite and >= 0 */
+static int valid_shifts(int nshifts, const double *shifts)
+{
+    if (nshifts < 1 || nshifts > ACGB200_MAXK || !shifts) return 0;
+    for (int j = 0; j < nshifts; j++) if (!(isfinite(shifts[j]) && shifts[j] >= 0)) return 0;
+    return 1;
+}
+
+/* r = p = b, X = 0 (X: c->d_x) and P_j = b */
+static int shifted_setup(struct solvectx *c)
+{
+    int *errcode = c->errcode;
+    KL(acgb200_shift_setup(c->pv->nowned, c->mk, c->d_b, c->cg->d_r, c->cg->d_p, c->d_x, c->pv->d_mp, c->pv->stream));
+    return ACG_SUCCESS;
 }
 
 /* the state of iteration 0: zeta_0 = zeta_{-1} = 1, alpha_{-1} = 1, beta_{-1} = 0 */
@@ -1912,28 +2002,15 @@ int acgsolvercuda_solve_shifted(struct acgsolvercuda *cg, const struct acgsymcsr
                                 struct acgb200_colstats *stats)
 {
     int errcode_ = 0, *errcode = &errcode_;
-    cfg_load();
-    struct priv *pv = priv_of(cg);
-    if (!pv) return ACG_ERR_INVALID_VALUE;
-    if (!have_shift_kernels() || !one_gpu(pv, A)) return ACG_ERR_NOT_SUPPORTED;
-    if (nshifts < 1 || nshifts > ACGB200_MAXK || !shifts || !b || !X || maxits < 0) return ACG_ERR_INVALID_VALUE;
-    for (int j = 0; j < nshifts; j++) if (!(isfinite(shifts[j]) && shifts[j] >= 0)) return ACG_ERR_INVALID_VALUE;
+    struct priv *pv;
+    OK(one_gpu_entry(cg, A, 1, have_shift_kernels(), valid_shifts(nshifts, shifts) && b && X && maxits >= 0, &pv));
     const int K = block_width(nshifts), n = pv->nowned;
     OK(ensure_blocks(pv, cg, K, errcode));
-    if (!pv->d_ss) {
-        CU(cudaMalloc((void **) &pv->d_ss, sizeof(*pv->d_ss)));
-        CU(cudaMallocHost((void **) &pv->h_ss, sizeof(*pv->h_ss)));
-    }
+    OK(dev_scalars_once(pv, (void **) &pv->d_ss, sizeof(*pv->d_ss), errcode));
     struct solvectx c;
-    memset(&c, 0, sizeof(c));
-    c.cg = cg; c.pv = pv; c.errcode = errcode; c.mk = K; c.kind = KIND_SHIFTED;
+    block_begin(&c, cg, pv, KIND_SHIFTED, K, X, nshifts, errcode);
     /* b lives in the first n entries of the B block, which this loop does not otherwise use */
-    double *const d_b = pv->d_mb;
-    c.d_b = d_b; c.d_x = pv->d_mx;
-    const double tb = wall();
-    CU(cudaMemcpyAsync(d_b, b, (size_t) n * sizeof(double), cudaMemcpyHostToDevice, pv->stream));
-    CU(cudaStreamSynchronize(pv->stream));
-    pv->last_h2d_ms = 1e3 * (wall() - tb);
+    OK(upload(&c, c.d_b, b, (size_t) n, 1, 1));
     struct acgb200_devstate h;
     struct acgb200_sstate ss;
     const unsigned all = (1u << nshifts) - 1u;
@@ -1941,13 +2018,13 @@ int acgsolvercuda_solve_shifted(struct acgsolvercuda *cg, const struct acgsymcsr
     /* warm-up: `warmup` iterations from the real set-up on state that is overwritten below; the R block
      * stands in for X, so X is untouched */
     if (warmup > 0) {
-        KL(acgb200_shift_setup(n, K, d_b, cg->d_r, cg->d_p, pv->d_mr, pv->d_mp, pv->stream));
+        c.d_x = pv->d_mr;
+        OK(shifted_setup(&c));
         sstate_init(&ss, nshifts, shifts, 0.0, 1.0);
-        OK(scalars_push(&c, pv->d_ss, pv->h_ss, &ss, sizeof(ss)));
+        OK(scalars_push(&c, pv->d_ss, &ss, sizeof(ss)));
         memset(&h, 0, sizeof(h));
         h.maxits = warmup; h.rr_loc[0] = h.rr[0] = 1.0; h.ctrl[0].pad0 = (int) all;
-        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
-        c.d_x = pv->d_mr;
+        OK(scalars_push(&c, pv->d_st, &h, sizeof(h)));
         for (int i = 0; i < warmup; i++) OK(shifted_iteration(&c, i));
         c.d_x = pv->d_mx;
         CU(cudaStreamSynchronize(pv->stream));
@@ -1955,53 +2032,36 @@ int acgsolvercuda_solve_shifted(struct acgsolvercuda *cg, const struct acgsymcsr
     OK(window_open(&c, maxits, residualatol, residualrtol, 0, 0));
 
     /* r0 = p0 = b (x0 = 0 for every shift), X = 0, P_j = b ; ||b|| */
-    memset(&h, 0, sizeof(h));
-    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
-    KL(acgb200_shift_setup(n, K, d_b, cg->d_r, cg->d_p, pv->d_mx, pv->d_mp, pv->stream));
-    KL(acgb200_dot(n, d_b, d_b, &pv->d_st->tmp_loc[0], pv->stream));
-    double bb = 0;
-    OK(reduce_to_host(&c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &bb));
+    double bb = 0, tol = 0, rtol_scaled[ACGB200_MAXK];
+    OK(rhs_norm(&c, shifted_setup, &bb));
     c.launches += 2;
     const double bnrm2 = sqrt(bb);
-    const double tol = threshold(residualatol, residualrtol, bnrm2);
-    const double rtol_scaled = residualrtol * bnrm2;
     /* every shifted system starts from r0 = b, so all meet the test at r0 or none does */
-    const unsigned mask = tol > 0 && bnrm2 < tol ? 0u : all;
+    const unsigned mask = r0_test(residualatol, residualrtol, bnrm2, &tol, &rtol_scaled[0]) ? 0u : all;
     int nits[ACGB200_MAXK], conv[ACGB200_MAXK];
-    double rn[ACGB200_MAXK];
-    for (int j = 0; j < nshifts; j++) { nits[j] = 0; conv[j] = !(mask >> j & 1u); rn[j] = bnrm2; }
+    double bbs[ACGB200_MAXK], rr[ACGB200_MAXK];
+    for (int j = 0; j < nshifts; j++) {
+        nits[j] = 0; conv[j] = !(mask >> j & 1u); bbs[j] = bb; rr[j] = bnrm2 * bnrm2; rtol_scaled[j] = rtol_scaled[0];
+    }
     if (maxits > 0 && mask) {
         sstate_init(&ss, nshifts, shifts, tol, bnrm2);
-        OK(scalars_push(&c, pv->d_ss, pv->h_ss, &ss, sizeof(ss)));
+        OK(scalars_push(&c, pv->d_ss, &ss, sizeof(ss)));
         memset(&h, 0, sizeof(h));
         h.maxits = maxits; h.rr_loc[0] = h.rr[0] = bb; h.ctrl[0].pad0 = (int) mask;
-        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_push(&c, pv->d_st, &h, sizeof(h)));
         OK(iterate(&c, maxits, tol > 0, shifted_iteration));
-        OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
-        OK(scalars_pull(&c, pv->d_ss, pv->h_ss, &ss, sizeof(ss)));
+        OK(scalars_pull(&c, pv->d_st, &h, sizeof(h)));
+        OK(scalars_pull(&c, pv->d_ss, &ss, sizeof(ss)));
         cg->niterations = h.ctrl[0].iter;
-        for (int j = 0; j < nshifts; j++) { nits[j] = ss.nits[j]; conv[j] = ss.conv[j]; rn[j] = ss.final_rnrm2[j]; }
-    }
-    cg->ntotaliterations += cg->niterations;
-    OK(window_close(&c));
-    account_shifted(cg, pv, cg->niterations, nshifts);
-    cg->ncopy += 2; cg->nnrm2++;
-    double sr = 0;
-    int status = ACG_SUCCESS;
-    for (int j = 0; j < nshifts; j++) {
-        sr += rn[j] * rn[j];
-        if (not_converged(conv[j], residualatol, rtol_scaled)) status = ACG_ERR_NOT_CONVERGED;      /* per shift */
-        if (stats) {
-            stats[j].niterations = nits[j]; stats[j].converged = conv[j];
-            stats[j].bnrm2 = bnrm2; stats[j].r0nrm2 = bnrm2; stats[j].rnrm2 = rn[j];
+        for (int j = 0; j < nshifts; j++) {
+            nits[j] = ss.nits[j]; conv[j] = ss.conv[j]; rr[j] = ss.final_rnrm2[j] * ss.final_rnrm2[j];
         }
     }
-    cg->bnrm2 = cg->r0nrm2 = sqrt((double) nshifts * bb); cg->rnrm2 = sqrt(sr);
-    const double te = wall();
-    OK(download_block_vec(pv, X, pv->d_mx, nshifts, K, errcode));
-    pv->last_d2h_ms = 1e3 * (wall() - te);
-    CU(cudaGetLastError());
-    return status;
+    account_shifted(cg, pv, cg->niterations, nshifts);
+    cg->ncopy += 2; cg->nnrm2++;
+    const int status = column_results(cg, nshifts, nits, conv, bbs, bbs, rr, residualatol, rtol_scaled, stats);
+    cg->bnrm2 = cg->r0nrm2 = sqrt((double) nshifts * bb);
+    return solve_finish(&c, status);
 }
 
 /* ------------------------------------------------------------------------ */
@@ -2012,20 +2072,6 @@ int acgsolvercuda_solve_shifted(struct acgsolvercuda *cg, const struct acgsymcsr
 static int have_minres_kernels(void)
 {
     return acgb200_minres_setup && acgb200_minres_lanczos && acgb200_minres_update;
-}
-
-/* r0 = b - A x into d_r with (r0,r0) folded in; *r0nrm2 = ||r0|| */
-static int minres_residual(struct solvectx *c, double *r0nrm2)
-{
-    struct priv *pv = c->pv;
-    struct acgb200_devstate h;
-    memset(&h, 0, sizeof(h));
-    OK(scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h)));
-    double rr = 0;
-    OK(apply_A(c, c->d_x, c->d_x, c->cg->d_r, c->d_b, SPMV_R_B_AX, &pv->d_st->tmp_loc[0], 0, 0, 0, -1));
-    OK(reduce_to_host(c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &rr));
-    *r0nrm2 = sqrt(rr);
-    return ACG_SUCCESS;
 }
 
 /* v_1 = r0 / beta_1 in d_r, v_0 = w_{-1} = w_0 = 0, and the scalars of the first iteration:
@@ -2040,11 +2086,11 @@ static int minres_start(struct solvectx *c, int maxits, double tol, double beta1
     struct acgb200_nstate ns;
     memset(&ns, 0, sizeof(ns));
     ns.beta[0] = beta1; ns.cs[0] = -1.0; ns.phibar[0] = beta1;
-    OK(scalars_push(c, pv->d_ns, pv->h_ns, &ns, sizeof(ns)));
+    OK(scalars_push(c, pv->d_ns, &ns, sizeof(ns)));
     struct acgb200_devstate h;
     memset(&h, 0, sizeof(h));
     h.maxits = maxits; h.tol = tol;
-    return scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h));
+    return scalars_push(c, pv->d_st, &h, sizeof(h));
 }
 
 /* iteration k: t = A v_k (+ alpha_k), u = t - alpha_k v_k - beta_k v_{k-1} (+ (u,u)), then the rotation, w_k, x
@@ -2085,20 +2131,12 @@ int acgsolvercuda_solve_minres(struct acgsolvercuda *cg, const struct acgsymcsrm
 {
     int errcode_ = 0;
     if (!errcode) errcode = &errcode_;
-    cfg_load();
-    struct priv *pv = priv_of(cg);
-    if (!pv || !A || !b || !x) return ACG_ERR_INVALID_VALUE;
-    if (!have_minres_kernels() || !one_gpu(pv, A)) return ACG_ERR_NOT_SUPPORTED;
-    if (maxits < 0) return ACG_ERR_INVALID_VALUE;
-    struct acgcomm null = null_comm();
+    struct priv *pv;
+    OK(one_gpu_entry(cg, A, A && b && x, have_minres_kernels(), maxits >= 0, &pv));
     struct solvectx c;
-    OK(solve_begin(&c, cg, A, b, x, 0.0, 0.0, &null, 0, errcode));
-    c.kind = KIND_MINRES;
+    OK(solve_begin(&c, cg, A, b, x, 0.0, 0.0, &one_gpu_comm, 0, KIND_MINRES, errcode));
     const int n = pv->nowned;
-    if (!pv->d_ns) {
-        CU(cudaMalloc((void **) &pv->d_ns, sizeof(*pv->d_ns)));
-        CU(cudaMallocHost((void **) &pv->h_ns, sizeof(*pv->h_ns)));
-    }
+    OK(dev_scalars_once(pv, (void **) &pv->d_ns, sizeof(*pv->d_ns), errcode));
     for (int i = 0; i < 2; i++)
         if (!pv->d_nw[i]) CU(cudaMalloc((void **) &pv->d_nw[i], ((size_t) pv->nvec + 2) * sizeof(double)));
     struct acgb200_devstate h;
@@ -2106,43 +2144,36 @@ int acgsolvercuda_solve_minres(struct acgsolvercuda *cg, const struct acgsymcsrm
 
     /* warm-up: the set-up and `warmup` iterations on x itself, then x0 again from the caller's vector */
     if (warmup > 0) {
-        double beta1 = 0;
-        OK(minres_residual(&c, &beta1));
-        OK(minres_start(&c, warmup, 0.0, beta1));
+        double rr = 0;
+        OK(residual(&c, &rr));
+        OK(minres_start(&c, warmup, 0.0, sqrt(rr)));
         for (int i = 0; i < warmup; i++) OK(minres_iteration(&c, i));
         OK(upload_x0(&c, x));
     }
     OK(window_open(&c, maxits, residualatol, residualrtol, 0, 0));
 
     /* ||b|| ; r0 = b - A x0 and beta_1 = ||r0|| */
-    memset(&h, 0, sizeof(h));
-    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
-    double bb = 0, beta1 = 0;
-    KL(acgb200_dot(n, c.d_b, c.d_b, &pv->d_st->tmp_loc[0], pv->stream));
-    OK(reduce_to_host(&c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &bb));
+    double bb = 0, rr0 = 0, tol = 0, rtol_scaled = 0;
+    OK(rhs_norm(&c, NULL, &bb));
     c.launches += 1;
-    cg->bnrm2 = sqrt(bb);
-    OK(minres_residual(&c, &beta1));
+    OK(residual(&c, &rr0));
+    const double beta1 = sqrt(rr0);
     cg->rnrm2 = cg->r0nrm2 = beta1;
     cg->nnrm2 += 2; cg->nflops += 4 * (int64_t) n; cg->Bnrm2 += 8 * (int64_t) n; cg->ngemv++;
-    const double tol = threshold(residualatol, residualrtol, beta1);
-    const double rtol_scaled = residualrtol * beta1;
-    int converged = tol > 0 && beta1 < tol;                        /* acg/cgcuda.c:836-842 */
+    int converged = r0_test(residualatol, residualrtol, beta1, &tol, &rtol_scaled);
 
     /* beta_1 = 0: x0 solves the system, there is no Krylov space to build */
     if (!converged && maxits > 0 && beta1 > 0) {
         OK(minres_start(&c, maxits, tol, beta1));
         OK(iterate(&c, maxits, tol > 0, minres_iteration));
-        OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
-        OK(scalars_pull(&c, pv->d_ns, pv->h_ns, &ns, sizeof(ns)));
+        OK(scalars_pull(&c, pv->d_st, &h, sizeof(h)));
+        OK(scalars_pull(&c, pv->d_ns, &ns, sizeof(ns)));
         cg->niterations = h.ctrl[0].iter;
         cg->rnrm2 = ns.phibar[cg->niterations & 1];
         converged = tol > 0 && cg->rnrm2 < tol;
-        cg->ntotaliterations += cg->niterations;
     }
-    OK(window_close(&c));
     account_minres(cg, pv, cg->niterations);
-    return solve_end(&c, x, not_converged(converged, residualatol, rtol_scaled) ? ACG_ERR_NOT_CONVERGED : ACG_SUCCESS);
+    return solve_finish(&c, convergence_status(converged, residualatol, rtol_scaled));
 }
 
 /* ------------------------------------------------------------------------ */
@@ -2159,10 +2190,7 @@ static int have_mixed_kernels(void)
 /* the float vectors (16 bytes per row), the scalars and the product's row chunks, made once per solver */
 static int mixed_alloc(struct priv *pv, const struct acgsolvercuda *cg, int *errcode)
 {
-    if (!pv->d_xs) {
-        CU(cudaMalloc((void **) &pv->d_xs, sizeof(*pv->d_xs)));
-        CU(cudaMallocHost((void **) &pv->h_xs, sizeof(*pv->h_xs)));
-    }
+    OK(dev_scalars_once(pv, (void **) &pv->d_xs, sizeof(*pv->d_xs), errcode));
     if (!pv->d_f32) {
         /* four vectors of nowned + 2 floats, each starting on an 8-byte boundary (the kernels read pairs) */
         const size_t bytes = 4 * (((size_t) pv->nowned + 2) & ~(size_t) 1) * sizeof(float);
@@ -2202,18 +2230,6 @@ static int apply_A_f32(struct solvectx *c, const float *x, float *y, double *acc
     return ACG_SUCCESS;
 }
 
-/* r64 = b - A x into d_r with (r64, r64) folded in (ungated) */
-static int mixed_residual(struct solvectx *c, double *rr)
-{
-    struct priv *pv = c->pv;
-    struct acgb200_devstate h;
-    memset(&h, 0, sizeof(h));
-    OK(scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h)));
-    *rr = 0;
-    OK(apply_A(c, c->d_x, c->d_x, c->cg->d_r, c->d_b, SPMV_R_B_AX, &pv->d_st->tmp_loc[0], 0, 0, 0, -1));
-    return reduce_to_host(c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, rr);
-}
-
 /* sigma = 2^round(log2 sqrt(rr)) as its exponent (as mixed_scale_exp of kernels.cu) */
 static int mixed_scale_exp(double rr)
 {
@@ -2235,11 +2251,11 @@ static int mixed_start(struct solvectx *c, int maxits, double tol, double rr64)
     memset(&xs, 0, sizeof(xs));
     xs.rho[0] = ldexp(rr64, -2 * e); xs.mx[0] = sqrt(xs.rho[0]); xs.sigma[0] = ldexp(1.0, e);
     xs.last_rr64 = rr64;
-    OK(scalars_push(c, pv->d_xs, pv->h_xs, &xs, sizeof(xs)));
+    OK(scalars_push(c, pv->d_xs, &xs, sizeof(xs)));
     struct acgb200_devstate h;
     memset(&h, 0, sizeof(h));
     h.maxits = maxits; h.tol = tol;
-    return scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h));
+    return scalars_push(c, pv->d_st, &h, sizeof(h));
 }
 
 /* iteration k: t = fl32(A p) (+ pi), r -= alpha t (+ rho'), y and p (or the fold), the fp64 residual and
@@ -2280,15 +2296,10 @@ int acgsolvercuda_solve_mixed(struct acgsolvercuda *cg, const struct acgsymcsrma
 {
     int errcode_ = 0;
     if (!errcode) errcode = &errcode_;
-    cfg_load();
-    struct priv *pv = priv_of(cg);
-    if (!pv || !A || !b || !x) return ACG_ERR_INVALID_VALUE;
-    if (!have_mixed_kernels() || !one_gpu(pv, A)) return ACG_ERR_NOT_SUPPORTED;
-    if (maxits < 0) return ACG_ERR_INVALID_VALUE;
-    struct acgcomm null = null_comm();
+    struct priv *pv;
+    OK(one_gpu_entry(cg, A, A && b && x, have_mixed_kernels(), maxits >= 0, &pv));
     struct solvectx c;
-    OK(solve_begin(&c, cg, A, b, x, 0.0, 0.0, &null, 0, errcode));
-    c.kind = KIND_MIXED;
+    OK(solve_begin(&c, cg, A, b, x, 0.0, 0.0, &one_gpu_comm, 0, KIND_MIXED, errcode));
     const int n = pv->nowned;
     OK(mixed_alloc(pv, cg, errcode));
     struct acgb200_devstate h;
@@ -2297,7 +2308,7 @@ int acgsolvercuda_solve_mixed(struct acgsolvercuda *cg, const struct acgsymcsrma
     /* warm-up: the set-up and `warmup` iterations on x itself, then x0 again from the caller's vector */
     if (warmup > 0) {
         double rr = 0;
-        OK(mixed_residual(&c, &rr));
+        OK(residual(&c, &rr));
         if (rr > 0) {
             OK(mixed_start(&c, warmup, 0.0, rr));
             for (int i = 0; i < warmup; i++) OK(mixed_iteration(&c, i));
@@ -2307,27 +2318,21 @@ int acgsolvercuda_solve_mixed(struct acgsolvercuda *cg, const struct acgsymcsrma
     OK(window_open(&c, maxits, residualatol, residualrtol, 0, 0));
 
     /* ||b|| ; r0 = b - A x0 in fp64 */
-    memset(&h, 0, sizeof(h));
-    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
-    double bb = 0, rr0 = 0;
-    KL(acgb200_dot(n, c.d_b, c.d_b, &pv->d_st->tmp_loc[0], pv->stream));
-    OK(reduce_to_host(&c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &bb));
+    double bb = 0, rr0 = 0, tol = 0, rtol_scaled = 0;
+    OK(rhs_norm(&c, NULL, &bb));
     c.launches += 1;
-    cg->bnrm2 = sqrt(bb);
-    OK(mixed_residual(&c, &rr0));
+    OK(residual(&c, &rr0));
     cg->rnrm2 = cg->r0nrm2 = sqrt(rr0);
     cg->nnrm2 += 2; cg->nflops += 4 * (int64_t) n; cg->Bnrm2 += 8 * (int64_t) n; cg->ngemv++;
-    const double tol = threshold(residualatol, residualrtol, cg->r0nrm2);
-    const double rtol_scaled = residualrtol * cg->r0nrm2;
-    int converged = tol > 0 && cg->rnrm2 < tol;                    /* acg/cgcuda.c:836-842 */
+    int converged = r0_test(residualatol, residualrtol, cg->r0nrm2, &tol, &rtol_scaled);
     int nupdates = 0;
 
     /* ||r0|| = 0: x0 solves the system */
     if (!converged && maxits > 0 && rr0 > 0) {
         OK(mixed_start(&c, maxits, tol, rr0));
         OK(iterate(&c, maxits, 1, mixed_iteration));
-        OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
-        OK(scalars_pull(&c, pv->d_xs, pv->h_xs, &xs, sizeof(xs)));
+        OK(scalars_pull(&c, pv->d_st, &h, sizeof(h)));
+        OK(scalars_pull(&c, pv->d_xs, &xs, sizeof(xs)));
         cg->niterations = h.ctrl[0].iter;
         nupdates = xs.nupdates;
         if (xs.conv || xs.breakdown) {
@@ -2337,18 +2342,16 @@ int acgsolvercuda_solve_mixed(struct acgsolvercuda *cg, const struct acgsymcsrma
             /* maxits: the last fold, then the residual of the x returned */
             KL(acgb200_mixed_fold(n, xs.sigma[cg->niterations & 1], mixed_vec(pv, 3), c.d_x, pv->stream));
             double rr = 0;
-            OK(mixed_residual(&c, &rr));
+            OK(residual(&c, &rr));
             c.launches += 1;
             cg->rnrm2 = sqrt(rr);
             cg->ngemv++;
         }
         converged = tol > 0 && cg->rnrm2 < tol;
-        cg->ntotaliterations += cg->niterations;
     }
-    OK(window_close(&c));
     account_mixed(cg, pv, cg->niterations, nupdates);
     pv->last_mixed_updates = nupdates;
-    return solve_end(&c, x, not_converged(converged, residualatol, rtol_scaled) ? ACG_ERR_NOT_CONVERGED : ACG_SUCCESS);
+    return solve_finish(&c, convergence_status(converged, residualatol, rtol_scaled));
 }
 
 /* ------------------------------------------------------------------------ */
@@ -2372,11 +2375,7 @@ static int cheb_alloc(struct solvectx *c)
     struct acgsolvercuda *cg = c->cg;
     struct priv *pv = c->pv;
     int *errcode = c->errcode;
-    if (!pv->d_cs) {
-        CU(cudaMalloc((void **) &pv->d_cs, sizeof(*pv->d_cs)));
-        CU(cudaMallocHost((void **) &pv->h_cs, sizeof(*pv->h_cs)));
-        pv->cheb_baddiag = -1;
-    }
+    OK(dev_scalars_once(pv, (void **) &pv->d_cs, sizeof(*pv->d_cs), errcode));
     if (!pv->d_cvec) {
         const size_t bytes = 5 * ((size_t) pv->nowned + 2) * sizeof(double);
         CU(cudaMalloc((void **) &pv->d_cvec, bytes));
@@ -2385,24 +2384,12 @@ static int cheb_alloc(struct solvectx *c)
     if (pv->cheb_baddiag < 0) {
         struct acgb200_cstate cs;
         memset(&cs, 0, sizeof(cs));
-        OK(scalars_push(c, pv->d_cs, pv->h_cs, &cs, sizeof(cs)));
+        OK(scalars_push(c, pv->d_cs, &cs, sizeof(cs)));
         KL(acgb200_cheb_dinv(pv->nowned, cg->d_rowptr, cg->d_colidx, cg->d_a, cheb_vec(pv, 0), pv->d_cs, pv->stream));
-        OK(scalars_pull(c, pv->d_cs, pv->h_cs, &cs, sizeof(cs)));
+        OK(scalars_pull(c, pv->d_cs, &cs, sizeof(cs)));
         pv->cheb_baddiag = cs.baddiag;
     }
     return ACG_SUCCESS;
-}
-
-/* r0 = b - A x into d_r with (r0,r0) folded in */
-static int cheb_residual(struct solvectx *c, double *rr)
-{
-    struct priv *pv = c->pv;
-    struct acgb200_devstate h;
-    memset(&h, 0, sizeof(h));
-    OK(scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h)));
-    *rr = 0;
-    OK(apply_A(c, c->d_x, c->d_x, c->cg->d_r, c->d_b, SPMV_R_B_AX, &pv->d_st->tmp_loc[0], 0, 0, 0, -1));
-    return reduce_to_host(c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, rr);
 }
 
 /* the start c0 = 1/theta and the steps' (rho_j rho_{j-1}, 2 rho_j / delta) of the interval [a, b] (Saad,
@@ -2463,19 +2450,19 @@ static int cheb_start(struct solvectx *c, int maxits, double tol, int log)
     struct acgb200_cstate cs;
     memset(&cs, 0, sizeof(cs));
     cs.log = log;
-    OK(scalars_push(c, pv->d_cs, pv->h_cs, &cs, sizeof(cs)));
+    OK(scalars_push(c, pv->d_cs, &cs, sizeof(cs)));
     struct acgb200_devstate h;
     memset(&h, 0, sizeof(h));
     h.maxits = maxits; h.tol = tol;
     h.ctrl[1].iter = h.ctrl[2].iter = -1;
-    OK(scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h)));
+    OK(scalars_push(c, pv->d_st, &h, sizeof(h)));
     KL(acgb200_cheb_rx(n, pv->d_st, pv->d_cs, 1, c->cheb_degree > 0, c->cheb_c0, cheb_vec(pv, 0), NULL, NULL, NULL,
                        c->cheb_r, cheb_vec(pv, 1), cheb_vec(pv, 2), cheb_vec(pv, 3), pv->stream));
     c->launches += 1;
     OK(cheb_steps(c));
     CU(cudaMemcpyAsync(cg->d_p, cheb_vec(pv, 1), (size_t) n * sizeof(double), cudaMemcpyDeviceToDevice, pv->stream));
     h.ctrl[1].iter = h.ctrl[2].iter = 0;
-    return scalars_push(c, pv->d_st, pv->h_st, &h, sizeof(h));
+    return scalars_push(c, pv->d_st, &h, sizeof(h));
 }
 
 /* iteration k: t = A p (+ (p, t)), the r/x kernel, the d inner steps, the p kernel */
@@ -2570,8 +2557,8 @@ static int cheb_estimate(struct solvectx *c, double tol, int *steps, double *the
     for (int i = 0; i < ACGB200_CHEB_EST; i++) OK(cheb_iteration(c, i));
     struct acgb200_devstate h;
     struct acgb200_cstate cs;
-    OK(scalars_pull(c, pv->d_st, pv->h_st, &h, sizeof(h)));
-    OK(scalars_pull(c, pv->d_cs, pv->h_cs, &cs, sizeof(cs)));
+    OK(scalars_pull(c, pv->d_st, &h, sizeof(h)));
+    OK(scalars_pull(c, pv->d_cs, &cs, sizeof(cs)));
     c->cheb_degree = degree; c->cheb_fused = fused; c->cheb_r = r; c->cheb_x = x;
     *steps = h.ctrl[0].iter;
     *theta_max = 0;
@@ -2607,18 +2594,14 @@ int acgsolvercuda_solve_chebyshev(struct acgsolvercuda *cg, const struct acgsymc
 {
     int errcode_ = 0;
     if (!errcode) errcode = &errcode_;
-    cfg_load();
-    struct priv *pv = priv_of(cg);
-    if (!pv || !A || !b || !x) return ACG_ERR_INVALID_VALUE;
-    if (!have_cheb_kernels() || !one_gpu(pv, A)) return ACG_ERR_NOT_SUPPORTED;
-    if (maxits < 0 || degree < 0 || degree > ACGB200_CHEB_MAXDEG) return ACG_ERR_INVALID_VALUE;
     /* the interval: non-negative and finite (0: estimated), a given lower bound below a given upper one */
-    if (degree > 0 && (!(isfinite(lmin) && lmin >= 0) || !(isfinite(lmax) && lmax >= 0) ||
-                       (lmin > 0 && lmax > 0 && lmin >= lmax))) return ACG_ERR_INVALID_VALUE;
-    struct acgcomm null = null_comm();
+    const int interval_ok = degree == 0 || (isfinite(lmin) && lmin >= 0 && isfinite(lmax) && lmax >= 0 &&
+                                            !(lmin > 0 && lmax > 0 && lmin >= lmax));
+    struct priv *pv;
+    OK(one_gpu_entry(cg, A, A && b && x, have_cheb_kernels(),
+                     maxits >= 0 && degree >= 0 && degree <= ACGB200_CHEB_MAXDEG && interval_ok, &pv));
     struct solvectx c;
-    OK(solve_begin(&c, cg, A, b, x, 0.0, 0.0, &null, 0, errcode));
-    c.kind = KIND_CHEB;
+    OK(solve_begin(&c, cg, A, b, x, 0.0, 0.0, &one_gpu_comm, 0, KIND_CHEB, errcode));
     const int n = pv->nowned;
     OK(cheb_alloc(&c));
     if (pv->cheb_baddiag != 0) return ACG_ERR_INVALID_VALUE;
@@ -2635,7 +2618,7 @@ int acgsolvercuda_solve_chebyshev(struct acgsolvercuda *cg, const struct acgsymc
      * vector */
     if (warmup > 0) {
         double rr = 0;
-        OK(cheb_residual(&c, &rr));
+        OK(residual(&c, &rr));
         if (rr > 0) {
             cheb_coefficients(&c, 0.2, 2.0);
             OK(cheb_start(&c, warmup, 0.0, 0));
@@ -2647,19 +2630,13 @@ int acgsolvercuda_solve_chebyshev(struct acgsolvercuda *cg, const struct acgsymc
     pv->last_cheb_degree = degree;
 
     /* ||b|| ; r0 = b - A x0 */
-    memset(&h, 0, sizeof(h));
-    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
-    double bb = 0, rr0 = 0;
-    KL(acgb200_dot(n, c.d_b, c.d_b, &pv->d_st->tmp_loc[0], pv->stream));
-    OK(reduce_to_host(&c, &pv->d_st->tmp_loc[0], &pv->d_st->tmp[0], 1, &bb));
+    double bb = 0, rr0 = 0, tol = 0, rtol_scaled = 0;
+    OK(rhs_norm(&c, NULL, &bb));
     c.launches += 1;
-    cg->bnrm2 = sqrt(bb);
-    OK(cheb_residual(&c, &rr0));
+    OK(residual(&c, &rr0));
     cg->rnrm2 = cg->r0nrm2 = sqrt(rr0);
     cg->nnrm2 += 2; cg->nflops += 4 * (int64_t) n; cg->Bnrm2 += 8 * (int64_t) n; cg->ngemv++;
-    const double tol = threshold(residualatol, residualrtol, cg->r0nrm2);
-    const double rtol_scaled = residualrtol * cg->r0nrm2;
-    int converged = tol > 0 && cg->rnrm2 < tol;                    /* acg/cgcuda.c:836-842 */
+    int converged = r0_test(residualatol, residualrtol, cg->r0nrm2, &tol, &rtol_scaled);
     int nsetup = 0;
 
     /* ||r0|| = 0: x0 solves the system */
@@ -2696,18 +2673,16 @@ int acgsolvercuda_solve_chebyshev(struct acgsolvercuda *cg, const struct acgsymc
             nsetup += degree;
             OK(iterate(&c, maxits, 1, cheb_iteration));
             struct acgb200_cstate cs;
-            OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
-            OK(scalars_pull(&c, pv->d_cs, pv->h_cs, &cs, sizeof(cs)));
+            OK(scalars_pull(&c, pv->d_st, &h, sizeof(h)));
+            OK(scalars_pull(&c, pv->d_cs, &cs, sizeof(cs)));
             cg->niterations = h.ctrl[0].iter;
             if (cg->niterations > 0) cg->rnrm2 = sqrt(h.final_rr);
             pv->last_cheb_breakdown = cs.breakdown;
         }
         converged = tol > 0 && cg->rnrm2 < tol;
-        cg->ntotaliterations += cg->niterations;
     }
-    OK(window_close(&c));
     account_cheb(cg, pv, cg->niterations, degree, c.cheb_fused, nsetup);
-    return solve_end(&c, x, not_converged(converged, residualatol, rtol_scaled) ? ACG_ERR_NOT_CONVERGED : ACG_SUCCESS);
+    return solve_finish(&c, convergence_status(converged, residualatol, rtol_scaled));
 }
 
 /* ------------------------------------------------------------------------ */
@@ -2799,7 +2774,7 @@ int acgsolvercuda_solve_pipelined(
     if (!errcode) errcode = &errcode_;
     cfg_load();
     struct solvectx c;
-    OK(solve_begin(&c, cg, A, b, x, diffatol, diffrtol, comm, tag, errcode));
+    OK(solve_begin(&c, cg, A, b, x, diffatol, diffrtol, comm, tag, KIND_PIPELINED, errcode));
     struct priv *pv = c.pv;
     struct acgb200_devstate *st = pv->d_st;
     const int n = pv->nowned;
@@ -2810,7 +2785,6 @@ int acgsolvercuda_solve_pipelined(
     OK(ensure_vec(&cg->q, &cg->d_q, A, pv->nvec, errcode));
     OK(ensure_vec(&cg->z, &cg->d_z, A, pv->nvec, errcode));
 
-    c.kind = KIND_PIPELINED;
     c.p2p = c.multi && pv->p2p.enabled && cfg.p2p;
     /* one kernel per iteration: one GPU, mirrored diagonals for the slice rows, all other rows in tiles */
     const struct acgb200_spmvplan *pl = &pv->plan;
@@ -2836,7 +2810,7 @@ int acgsolvercuda_solve_pipelined(
         memset(&h, 0, sizeof(h));
         h.maxits = warmup;
         for (int s = 0; s < 2; s++) { h.gd_loc[s][0] = h.gd[s][0] = 1; h.gd_loc[s][1] = h.gd[s][1] = 1; h.prev[s][0] = h.prev[s][1] = INFINITY; }
-        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_push(&c, pv->d_st, &h, sizeof(h)));
         /* x on r: the fused loop also writes the r ring, and the set-up below rewrites every slot before the
          * solve reads it (d_r from b - A x0, slot j in iteration j - 1) */
         double *xsave = c.d_x; c.d_x = cg->d_r;
@@ -2857,12 +2831,8 @@ int acgsolvercuda_solve_pipelined(
     CU(cudaMemsetAsync(cg->d_w, 0, ((size_t) pv->nvec + 2) * sizeof(double), pv->stream));
     OK(window_open(&c, maxits, residualatol, residualrtol, diffatol, diffrtol));
 
-    memset(&h, 0, sizeof(h));
-    OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
     double bb = 0, gd0[2] = { 0, 0 };
-    KL(acgb200_dot(n, c.d_b, c.d_b, &st->tmp_loc[0], pv->stream));
-    OK(reduce_to_host(&c, &st->tmp_loc[0], &st->tmp[0], 1, &bb));
-    cg->bnrm2 = sqrt(bb);
+    OK(rhs_norm(&c, NULL, &bb));
 
     /* r0 = b - A x0 ; w0 = A r0 (acg/cgcuda.c:1577-1671) */
     OK(apply_A(&c, c.d_x, c.d_x, cg->d_r, c.d_b, SPMV_R_B_AX, NULL, 0, 0, 0, -1));
@@ -2872,18 +2842,18 @@ int acgsolvercuda_solve_pipelined(
      * of the update kernel */
     KL(acgb200_dot2(n, cg->d_r, cg->d_w, &st->gd_loc[0][0], pv->stream));
     OK(reduce_to_host(&c, &st->gd_loc[0][0], &st->gd[0][0], 2, gd0));
+    /* the loop makes the stopping test, from iteration 0 on */
     int converged = 0;
-    double rtol_scaled = residualrtol;
+    double rtol_scaled = residualrtol, tol = 0;
     if (maxits > 0) {
         cg->rnrm2 = cg->r0nrm2 = sqrt(gd0[0]);                     /* acg/cgcuda.c:1760-1761 */
-        rtol_scaled = residualrtol * cg->r0nrm2;
-        const double tol = threshold(residualatol, residualrtol, cg->r0nrm2);
+        (void) r0_test(residualatol, residualrtol, cg->r0nrm2, &tol, &rtol_scaled);
         memset(&h, 0, sizeof(h));
         h.maxits = maxits; h.tol = tol;
         h.gd_loc[0][0] = h.gd[0][0] = gd0[0];
         h.gd_loc[0][1] = h.gd[0][1] = gd0[1];
         h.prev[0][0] = h.prev[0][1] = INFINITY;                    /* acg/cgcuda.c:1513-1514 */
-        OK(scalars_push(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_push(&c, pv->d_st, &h, sizeof(h)));
         if (c.p2p) {
             /* w_0 goes to the neighbours' windows as exchange number 0 */
             OK(acgb200_p2p_begin(&pv->p2p, maxits, pv->stream));
@@ -2897,7 +2867,7 @@ int acgsolvercuda_solve_pipelined(
                                         c.d_x, pv->stream));
             c.launches += 1;
         }
-        OK(scalars_pull(&c, pv->d_st, pv->h_st, &h, sizeof(h)));
+        OK(scalars_pull(&c, pv->d_st, &h, sizeof(h)));
         const struct acgb200_ctrl cw = h.ctrl[c.fused ? c.issued & 1 : 0];
         cg->niterations = cw.iter;
         converged = cw.done;
@@ -2907,9 +2877,7 @@ int acgsolvercuda_solve_pipelined(
         const double g = converged ? h.final_rr
             : (kk == 0 ? gd0[0] : (c.multi ? h.gd[kk & 1][0] : h.gd_loc[c.fused ? kk % 3 : kk & 1][0]));
         cg->rnrm2 = sqrt(g);
-        cg->ntotaliterations += cg->niterations;
     }
-    OK(window_close(&c));
     {
         const int64_t nits = cg->niterations, nnz = pv->fnnz + pv->onnz;
         const int64_t bgemv = nnz * 12 + (int64_t) n * 16 + (int64_t) (pv->nborder + pv->nghost) * 8 + (int64_t) pv->nvec * 8;
@@ -2922,7 +2890,7 @@ int acgsolvercuda_solve_pipelined(
             cg->nhalomsgs += (nits + 2) * cg->halo->nrecipients;
         }
     }
-    return solve_end(&c, x, not_converged(converged, residualatol, rtol_scaled) ? ACG_ERR_NOT_CONVERGED : ACG_SUCCESS);
+    return solve_finish(&c, convergence_status(converged, residualatol, rtol_scaled));
 }
 
 /* ------------------------------------------------------------------------ */
@@ -3246,8 +3214,7 @@ int acgsolvercuda_spmv_f32(struct acgsolvercuda *cg, const float *x, float *y, d
     CU(cudaMemsetAsync(mixed_vec(pv, 2), 0xff, (size_t) n * sizeof(float), pv->stream));
     CU(cudaMemsetAsync(&st->tmp_loc[0], 0, sizeof(double), pv->stream));
     struct solvectx c;
-    memset(&c, 0, sizeof(c));
-    c.cg = cg; c.pv = pv; c.errcode = errcode;
+    ctx_init(&c, cg, pv, errcode);
     OK(apply_A_f32(&c, mixed_vec(pv, 1), mixed_vec(pv, 2), &st->tmp_loc[0], 0));
     double hdot = 0;
     CU(cudaMemcpyAsync(y, mixed_vec(pv, 2), (size_t) n * sizeof(float), cudaMemcpyDeviceToHost, pv->stream));
@@ -3273,15 +3240,15 @@ int acgsolvercuda_spmm_mode(struct acgsolvercuda *cg, int mode, int nrhs, const 
     if (mode == SPMV_R_B_AX && !B) return ACG_ERR_INVALID_VALUE;
     const int K = block_width(nrhs), n = pv->nowned;
     OK(ensure_blocks(pv, cg, K, errcode));
-    OK(upload_block_vec(pv, pv->d_mp, X, nrhs, K, errcode));
-    if (mode == SPMV_R_B_AX) OK(upload_block_vec(pv, pv->d_mb, B, nrhs, K, errcode));
+    OK(upload_block_vec(pv, pv->d_mp, X, (size_t) n, nrhs, K, errcode));
+    if (mode == SPMV_R_B_AX) OK(upload_block_vec(pv, pv->d_mb, B, (size_t) n, nrhs, K, errcode));
     CU(cudaMemsetAsync(pv->d_mt, 0xff, (size_t) n * K * sizeof(double), pv->stream));
     CU(cudaMemsetAsync(&pv->d_ms->tmp[0], 0, sizeof(pv->d_ms->tmp), pv->stream));
     struct solvectx c;
-    memset(&c, 0, sizeof(c));
-    c.cg = cg; c.pv = pv; c.errcode = errcode; c.mk = K;
+    ctx_init(&c, cg, pv, errcode);
+    c.mk = K;
     OK(apply_A_multi(&c, pv->d_mp, pv->d_mt, mode == SPMV_R_B_AX ? pv->d_mb : NULL, mode, &pv->d_ms->tmp[0], 0));
-    OK(download_block_vec(pv, Y, pv->d_mt, nrhs, K, errcode));
+    OK(download_block_vec(pv, Y, pv->d_mt, (size_t) n, nrhs, K, errcode));
     double h[ACGB200_MAXK];
     CU(cudaMemcpy(h, &pv->d_ms->tmp[0], sizeof(h), cudaMemcpyDeviceToHost));
     if (dots) for (int j = 0; j < nrhs; j++) dots[j] = h[j];
